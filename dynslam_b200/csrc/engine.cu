@@ -97,6 +97,7 @@ static b200_status download_sync(b200_engine *e, b200_scene *s, b200_render_stat
 extern "C" {
 
 static b200_status engine_create_body(const b200_engine_config *cfg, b200_engine *e);
+static void read_switches(b200_engine *e);
 
 static thread_local char g_createErr[512] = "";
 
@@ -116,7 +117,6 @@ b200_status b200_engine_create(const b200_engine_config *cfg, b200_engine **out)
 }
 
 static b200_status engine_create_body(const b200_engine_config *cfg, b200_engine *e) {
-  e->useGraph = -1;
   e->maxRenderingBlocks = B200_MAX_RENDERING_BLOCKS;
   e->device = cfg->device;
   e->numBlocks = cfg->numBlocks; e->numBuckets = cfg->numBuckets; e->excessSize = cfg->excessSize;
@@ -179,13 +179,31 @@ static b200_status engine_create_body(const b200_engine_config *cfg, b200_engine
     CK(cudaEventCreateWithFlags(&e->evJoin, cudaEventDisableTiming));
   }
   e->hostAuthoritative = true;
+  read_switches(e);
   integrate_init_device(e);     // per-device tables and function attributes of integrate.cu (one engine per GPU is the multi-GPU unit)
   CK(cudaGetLastError());
+  return B200_OK;
+}
+
+// The run-time switches (README) are read once per engine, here: an engine keeps the values it was created with, and an
+// engine created after a variable was set or removed gets the new value (nothing is remembered per process).
+static void read_switches(b200_engine *e) {
+  const char *v;
   // default: V4 (packed-pair arithmetic, integrate.cu); B200_INTEGRATE_IMPL = v3 | tma | ldg select the earlier bit-exact variants,
   // fast = V4 in tolerance mode (TSDF within 1 LSB of the 16-bit code, everything else bit-exact)
-  { const char *v = getenv("B200_INTEGRATE_IMPL");
-    e->integrateImpl = !v ? 3 : (v[0] == 'l' ? 0 : (v[0] == 't' ? 1 : (v[0] == 'f' ? 4 : ((v[0] == 'v' && v[1] == '3') ? 2 : 3)))); }
-  return B200_OK;
+  v = getenv("B200_INTEGRATE_IMPL");
+  e->integrateImpl = !v ? 3 : (v[0] == 'l' ? 0 : (v[0] == 't' ? 1 : (v[0] == 'f' ? 4 : ((v[0] == 'v' && v[1] == '3') ? 2 : 3))));
+  v = getenv("B200_V4_PPL"); e->pplV4 = (v && (atoi(v) == 1 || atoi(v) == 2)) ? atoi(v) : 0;
+  v = getenv("B200_V4_TAIL"); e->v4TailFloor = (v && atoi(v) >= 1 && atoi(v) <= 6) ? atoi(v) : 3;
+  v = getenv("B200_V3_PREFETCH"); e->v3Prefetch = v ? atoi(v) != 0 : true;
+  v = getenv("B200_V3_CTAS"); e->ctasV3 = (v && (atoi(v) == 2 || atoi(v) == 4)) ? atoi(v) : 3;   // 3: 72 registers per thread; 4 = 56, 2 = 96
+  v = getenv("B200_INTEGRATE_REGS"); e->regsTma = (v && atoi(v) == 56) ? 56 : 48;
+  v = getenv("B200_INTEGRATE_CTAS"); e->ctasTma = v ? atoi(v) : 0;   // an upper bound; integrate_init_device sets the count
+  v = getenv("B200_RC_TILE"); e->rcTileLog2 = v ? atoi(v) : 3; if (e->rcTileLog2 < 0 || e->rcTileLog2 > 5) e->rcTileLog2 = 3;
+  v = getenv("B200_RC_ORDER"); e->rcOrder = v ? atoi(v) : 1;
+  v = getenv("B200_RC_IMPL"); e->rcImpl = (v && v[0] == 'o') ? 0 : 1;
+  v = getenv("B200_GRAPH"); e->useGraph = (v && atoi(v) != 0) ? 1 : 0;
+  e->lastIntegrateKernel = -1; e->lastIntegrateGrid = 0;
 }
 
 void b200_engine_destroy(b200_engine *e) {
@@ -255,6 +273,11 @@ int b200_get_trace(b200_engine *e, char *out, int cap) {
 }
 
 void b200_diag_set_max_rendering_blocks(b200_engine *e, int n) { e->maxRenderingBlocks = n > 0 ? n : B200_MAX_RENDERING_BLOCKS; }
+
+void b200_diag_last_integrate(const b200_engine *e, int *kernel, int *grid) {
+  if (kernel) *kernel = e->lastIntegrateKernel;
+  if (grid) *grid = e->lastIntegrateGrid;
+}
 
 int b200_diag_read_debug(b200_engine *e, unsigned long long *out, int n) {
   if (!e || !out || n <= 0) return 0;
@@ -527,7 +550,6 @@ b200_status b200_process_frame_async(b200_engine *e, b200_scene *s, b200_render_
   b200_status st = check_scene(e, s); if (st) return st;
   CK(cudaSetDevice(e->device));
   if (e->hostAuthoritative) { st = upload(e, s, rs); if (st) return st; e->hostAuthoritative = false; }
-  if (e->useGraph < 0) { const char *g = getenv("B200_GRAPH"); e->useGraph = (g && atoi(g) != 0) ? 1 : 0; }
   if (!e->useGraph || e->timing || e->traceOn || !e->graphWarm) {   // (events recorded inside a capture cannot be synchronised on)   // the first frame also runs one-time initialisation: never captured
     e->graphWarm = true;
     return frame_enqueue(e, s, rs, v, d_points, d_normals, opts);

@@ -318,15 +318,12 @@ k_raycast(float4 *out, const b200_voxel *__restrict__ voxels, const b200_hash_en
 
 void launch_raycast(b200_engine *e, const SceneRef &s, const Mat4 &invM, const float proj[4], int w, int h, float voxelSize, float mu,
                     const b200_vec2f *minmax, b200_vec4f *out) {
-  static int twLog2 = -1;
-  if (twLog2 < 0) { const char *v = getenv("B200_RC_TILE"); twLog2 = v ? atoi(v) : 3; if (twLog2 < 0 || twLog2 > 5) twLog2 = 3; }   // 3: 8x4 (default)
+  const int twLog2 = e->rcTileLog2;   // warp tile (1 << twLog2) x (32 >> twLog2) pixels; 3: 8x4 (default)
   const int tw = 1 << twLog2, th = 32 >> twLog2;
   const int tiles = ((w + tw - 1) / tw) * ((h + th - 1) / th);
   const int warpsPerCta = RC_THREADS / 32;
-  static int order = -1;
-  if (order < 0) { const char *v = getenv("B200_RC_ORDER"); order = v ? atoi(v) : 1; }   // default: principal-point row first; 0 = plain row-major
   int centreRow = -1;
-  if (order == 1) {   // principal-point row first (level camera: the horizon)
+  if (e->rcOrder == 1) {   // principal-point row first (level camera: the horizon); 0 = plain row-major
     const int tilesY = (h + th - 1) / th;
     centreRow = (int)(proj[3] / (float)th);
     if (centreRow < 0) centreRow = 0;
@@ -334,8 +331,7 @@ void launch_raycast(b200_engine *e, const SceneRef &s, const Mat4 &invM, const f
   }
   const int tilesXh = (w + tw - 1) / tw, tilesYh = (h + th - 1) / th;
   const unsigned magic = (unsigned)((0x100000000ull + (unsigned)tilesXh - 1) / (unsigned)tilesXh);
-  static int impl = -1;
-  if (impl < 0) { const char *v = getenv("B200_RC_IMPL"); impl = (v && v[0] == 'o') ? 0 : 1; }   // "old": per-lane one-entry cache (cross-check); default: neighbourhood cache
+  const int impl = e->rcImpl;   // 1: neighbourhood cache (default); 0: per-lane one-entry cache (cross-check)
   trace_begin(e, e->stream, "k_raycast");
   if (impl)
     k_raycast<true><<<(tiles + warpsPerCta - 1) / warpsPerCta, RC_THREADS, 0, e->stream>>>((float4 *)out, s.voxels, s.hash, s.numBuckets, w, h, invM,

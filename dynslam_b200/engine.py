@@ -221,6 +221,13 @@ class Engine:
         """test hook (include/b200fusion_diag.h): lower MAX_RENDERING_BLOCKS to reach the cap rule with small scenes"""
         self.lib.b200_diag_set_max_rendering_blocks(self.h, int(n))
 
+    def last_integrate(self):
+        """test hook (include/b200fusion_diag.h): (kernel, grid) of the last integrate launch; kernel 0 LDG, 1 TMA, 2 V3, 3 V4 with
+        two voxels per lane, 4 V4 with four, + 8 in tolerance mode"""
+        k, g = C.c_int(), C.c_int()
+        self.lib.b200_diag_last_integrate(self.h, C.byref(k), C.byref(g))
+        return k.value, g.value
+
     # ---- fused fast path --------------------------------------------------------------------
     def process_frame_async(self, renderState, view, points=None, normals=None, decay=None, raycast=True, colour_out=None,
                             depth_out=None):

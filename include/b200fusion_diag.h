@@ -42,6 +42,11 @@ b200_status b200_selftest_divide(b200_engine *e, uint64_t pairs, uint64_t seed, 
    (Vis_CUDA.cu:609) with small scenes. n <= 0 restores the reference's constant. */
 void b200_diag_set_max_rendering_blocks(b200_engine *e, int n);
 
+/* The IntegrateIntoScene kernel that this engine's last integrate launch ran, and its grid (CTAs): 0 = LDG, 1 = TMA, 2 = V3,
+   3 = V4 with two voxels per lane, 4 = V4 with four voxels per lane; + 8 in tolerance mode (B200_INTEGRATE_IMPL=fast).
+   -1 and 0 before the first launch. Tests use it to check that the variant they mean to exercise really ran. */
+void b200_diag_last_integrate(const b200_engine *e, int *kernel, int *grid);
+
 /* While the launch trace is on (b200_set_timing(e, 3)) a few CTAs of the allocation's list pass stamp %globaltimer at their
    phase boundaries (8 stamps x 4 CTAs, nanoseconds); copies up to 64 of them out. Measurement only. */
 int b200_diag_read_debug(b200_engine *e, unsigned long long *out, int n);

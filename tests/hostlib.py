@@ -214,8 +214,9 @@ class HostVolume:
                     lastFreeExcessListId=self.scene.lastFreeExcessListId)
 
 
-def make_view(depth, rgb, M_d, proj, M_rgb=None, depthWeighting=0, requiresFullRendering=1, inv=None):
-    """Host-pointer b200_view. Keeps references to the arrays on the returned object."""
+def make_view(depth, rgb, M_d, proj, M_rgb=None, depthWeighting=0, requiresFullRendering=1, inv=None, proj_rgb=None):
+    """Host-pointer b200_view. Keeps references to the arrays on the returned object. M_rgb / proj_rgb default to the depth
+    camera's."""
     L = oracle()
     depth = np.ascontiguousarray(depth, dtype=np.float32)
     rgb = np.ascontiguousarray(rgb, dtype=np.uint8)
@@ -229,8 +230,8 @@ def make_view(depth, rgb, M_d, proj, M_rgb=None, depthWeighting=0, requiresFullR
     v.invM_d = invc
     v.M_rgb = abi.mat_to_c(M_rgb if M_rgb is not None else M_d)
     v.proj_d = abi.f4(*[float(x) for x in proj])
-    v.proj_rgb = abi.f4(*[float(x) for x in proj])
-    v.depthWeighting, v.requiresFullRendering = depthWeighting, requiresFullRendering
+    v.proj_rgb = abi.f4(*[float(x) for x in (proj_rgb if proj_rgb is not None else proj)])
+    v.depthWeighting, v.requiresFullRendering = depthWeighting, int(requiresFullRendering)
     v._keep = (depth, rgb)
     return v
 

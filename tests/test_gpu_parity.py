@@ -101,37 +101,9 @@ def test_integrate_tolerance_mode():
     contracted sums). north_star's bar: allocation / indices bit-exact, TSDF and weights within 1e-5 — the weight, the depth pixel
     every voxel samples and the colours are still computed exactly; the TSDF is stored as a 16-bit code, so a result on the
     other side of a rounding boundary shows as 1 LSB (3.05e-5): counted here, must be rare and never more than 1 LSB.
-    Every frame starts from the oracle's voxels, so the figures are per integration step."""
-    os.environ["B200_INTEGRATE_IMPL"] = "fast"
-    try:
-        cfg = P.Cfg(frames=5, raycast=False)
-        pair = P.Pair(cfg)
-        L = pair.L
-        changed = flips = gate = 0
-        for i, (depth, rgb, M, proj) in enumerate(P.frames_of(cfg)):
-            gv, hv = pair.views(depth, rgb, M, proj)
-            pair.reco.AllocateSceneFromDepth(pair.scene, gv, pair.rs)
-            assert L.oracle_allocate_from_depth(pair.host.engine, C.byref(pair.host.scene), C.byref(pair.host.rs), C.byref(hv), 0, 0) == 0
-            pair.compare_scene(f"frame {i} allocate", voxels=False)          # hash, lists, visibility, counters: bit-exact
-            before = pair.host.voxels.copy()
-            pair.reco.IntegrateIntoScene(pair.scene, gv, pair.rs)
-            L.oracle_integrate(pair.host.engine, C.byref(pair.host.scene), C.byref(pair.host.rs), C.byref(hv), 0)
-            g, o = pair.scene.to_host()["voxels"], pair.host.voxels
-            assert np.array_equal(g["w_depth"], o["w_depth"])                # which voxels were updated, and their weights
-            ds = g["sdf"].astype(np.int32) - o["sdf"].astype(np.int32)
-            assert np.abs(ds).max() <= 1
-            upd = (o["sdf"] != before["sdf"]) | (o["w_depth"] != before["w_depth"])
-            changed += int(upd.sum()); flips += int((ds != 0).sum())
-            colour_diff = (g["clr"] != o["clr"]).any(axis=1) | (g["w_color"] != o["w_color"])
-            gate += int(colour_diff.sum())
-            assert np.abs(g["sdf"].astype(np.float32) / 32767.0 - o["sdf"].astype(np.float32) / 32767.0).max() <= 3.06e-5
-            pair.scene.voxels.copy_(torch.from_numpy(pair.host.voxels.view(np.uint8).reshape(-1)).to(pair.scene.device))
-        assert changed > 100000
-        assert flips < 0.02 * changed, (flips, changed)                      # a TSDF code on the other side of a rounding boundary
-        assert gate < 0.002 * changed, (gate, changed)                       # colour gate |eta/mu| <= 0.25 decided differently on a tie
-        print(f"tolerance mode: {changed} voxel updates, {flips} TSDF codes off by one LSB, {gate} colour-gate flips")
-    finally:
-        os.environ.pop("B200_INTEGRATE_IMPL", None)
+    Every frame starts from the oracle's voxels, so the figures are per integration step. (The four-voxel form:
+    tests/test_gpu_variants.py.)"""
+    P.check_tolerance_mode()
 
 
 def test_integrate_tma_variant_matches():
@@ -152,17 +124,17 @@ def test_integrate_wide_band_colour_on_rejected_voxels():
 
 
 def test_integrate_four_resident_ctas_build():
+    os.environ["B200_INTEGRATE_IMPL"] = "v3"
     os.environ["B200_V3_CTAS"] = "4"
     try:
-        # the register-budget switch is read once per process: run in a child
-        import subprocess, sys
-        code = ("from tests import parity as P; pair,_=P.run_sequence(P.Cfg(frames=4, raycast=False, decay=(1, 2))); "
-                "assert pair.rs.noVisibleBlocks > 1000; print('ok')")
-        out = subprocess.run([sys.executable, "-c", code], cwd=os.path.dirname(os.path.dirname(os.path.abspath(__file__))),
-                             capture_output=True, text=True, timeout=600)
-        assert out.returncode == 0 and "ok" in out.stdout, out.stdout + out.stderr
+        pair = P.Pair(P.Cfg(frames=4, raycast=False, decay=(1, 2)))   # the switches are read when the engine is created
     finally:
+        os.environ.pop("B200_INTEGRATE_IMPL", None)
         os.environ.pop("B200_V3_CTAS", None)
+    for i, f in enumerate(P.frames_of(pair.cfg)):
+        pair.step(*f, i)
+    assert pair.rs.noVisibleBlocks > 1000
+    assert pair.eng.last_integrate() == (2, 4 * torch.cuda.get_device_properties(0).multi_processor_count)
 
 
 def test_division_sequences_equal_ieee_division():

@@ -132,6 +132,56 @@ def test_integrate_blocks_bit_exact(seq):
     refpins.check("oracle_vs_ref/integrate_blocks", b"".join(ours), b"".join(refs) if R else None)
 
 
+def test_integrate_blocks_approximate_and_colour_camera_bit_exact():
+    """the two integration branches the default views never take: approximate integration (requiresFullRendering = false: only
+    voxels with w_depth == 0 are updated) and a colour camera of its own (M_rgb, proj_rgb and an RGB image size that differ from
+    the depth camera's: colours are re-projected). Frame 0 fills the volume with the default view, frames 1-3 use the branches."""
+    L, R = H.oracle(), _ref_or_none()
+    scene = synth.StreetScene(seed=6, length_m=80.0)
+    w, h = int(round(synth.KITTI_W * SCALE)), int(round(synth.KITTI_H * SCALE))
+    vol = H.HostVolume(20000, NB, NE, w, h, H.SceneParams(voxelSize=0.05, mu=0.75, maxW=50))
+    offset = np.array([[0.9998, -0.0050, 0.0200, -0.54], [0.0054, 0.9999, -0.0100, 0.05], [-0.0199, 0.0101, 0.9998, 0.02],
+                       [0, 0, 0, 1]], dtype=np.float64)
+    proj_rgb = np.array([707.0912 * 0.3, 707.0912 * 0.3, 601.8873 * 0.3 + 4.0, 183.1104 * 0.3 - 2.5], dtype=np.float32)
+    rng = np.random.RandomState(5)
+    ours, refs = [], []
+    kept = written = recoloured = 0
+    for f, (approx, own_rgb) in enumerate(((False, False), (True, False), (False, True), (True, True))):
+        depth, rgb, M, proj = synth.kitti_frame(scene, f * 2, scale=SCALE)
+        M_rgb, pr = None, None
+        if own_rgb:
+            M_rgb, pr = (offset @ M.astype(np.float64)).astype(np.float32), proj_rgb
+            rgb = scene.render(M_rgb, 373, 113, *[float(x) for x in pr])[1]
+        view = H.make_view(depth, rgb, M, proj, M_rgb=M_rgb, proj_rgb=pr, requiresFullRendering=int(not approx))
+        assert L.oracle_allocate_from_depth(vol.engine, C.byref(vol.scene), C.byref(vol.rs), C.byref(view), 0, 0) == 0
+        pre = vol.voxels.copy()
+        L.oracle_integrate(vol.engine, C.byref(vol.scene), C.byref(vol.rs), C.byref(view), 0)
+        if f == 0:
+            continue
+        vis = vol.visiblePos[:vol.rs.noVisibleBlocks]
+        for i in rng.choice(len(vis), size=min(300, len(vis)), replace=False):
+            x, y, z = (int(t) for t in vis[i])
+            idx = L.oracle_find_block(H.vptr(vol.hash), NB, x, y, z)
+            if idx < 0:
+                continue
+            ptr = int(vol.hash[idx]["ptr"])
+            a, b = pre[ptr * 512:(ptr + 1) * 512], vol.voxels[ptr * 512:(ptr + 1) * 512]
+            ours.append(b.tobytes())
+            if approx:
+                kept += int(((a["w_depth"] != 0) & (a["w_depth"] == b["w_depth"])).sum())
+                written += int(((a["w_depth"] == 0) & (b["w_depth"] != 0)).sum())
+            if own_rgb:
+                recoloured += int((a["clr"] != b["clr"]).any(axis=1).sum())
+            if R:
+                blk = a.copy()
+                pos = np.array([x, y, z], dtype=np.int16)
+                R.ref_integrate_block(H.vptr(blk), H.vptr(pos), C.byref(vol.scene), C.byref(view))
+                assert blk.tobytes() == b.tobytes(), (f, x, y, z)
+                refs.append(blk.tobytes())
+    assert kept > 10000 and written > 1000 and recoloured > 10000, (kept, written, recoloured)
+    refpins.check("oracle_vs_ref/integrate_blocks_approx_colour_camera", b"".join(ours), b"".join(refs) if R else None)
+
+
 def test_block_visibility_and_projection(seq):
     vol, frames = seq
     L, R = _hooks(), _ref_or_none()
