@@ -159,7 +159,7 @@ EXPORTS = [
 ]
 # measurement / test hooks (include/b200fusion_diag.h): exported by the same library, not part of the drop-in boundary
 DIAG_EXPORTS = ["b200_set_timing", "b200_get_trace", "b200_get_stats", "b200_selftest_divide", "b200_diag_set_max_rendering_blocks",
-                "b200_diag_read_debug", "b200_diag_last_integrate"]
+                "b200_diag_read_debug", "b200_diag_last_integrate", "b200_diag_push_decay_snapshot", "b200_diag_set_frame_index"]
 
 _lib = None
 
@@ -241,6 +241,9 @@ def load_library():
     lib.b200_diag_read_debug.argtypes = [vp, P(C.c_uint64), C.c_int]
     lib.b200_diag_last_integrate.argtypes = [vp, P(C.c_int), P(C.c_int)]
     lib.b200_diag_last_integrate.restype = None
+    lib.b200_diag_push_decay_snapshot.argtypes = [vp, vp, C.c_int]
+    lib.b200_diag_set_frame_index.argtypes = [vp, C.c_int32]
+    lib.b200_diag_set_frame_index.restype = None
     _lib = lib
     return lib
 

@@ -595,9 +595,7 @@ k_serve_list(const float *__restrict__ depth, b200_hash_entry *table, int numBuc
         const int kept = n < capacity ? n : capacity;
         // (a snapshot that wraps onto older live ones simply overwrites them: decay.cu recognises an overwritten snapshot by
         // ringHead - snapStart > ringCap when its turn comes and sweeps nothing — the oldest snapshots are dropped, never an error)
-        snapStart[slot] = ringStart;
-        snapCount[slot] = kept;
-        ctr->ringHead = ringStart + kept;
+        publish_snapshot(ctr, snapStart, snapCount, slot, ringStart, kept);
       }
       __syncthreads();
       if (threadIdx.x == 0) {

@@ -340,6 +340,21 @@ __global__ void k_find_allocated(const b200_hash_entry *__restrict__ table, int 
   }
 }
 
+// b200_diag_push_decay_snapshot: n caller positions appended to the ring as snapshot `slot` (one CTA: the cursor is read
+// before and moved after every item is written)
+__global__ void k_push_snapshot(const b200_vec3i *positions, int n, b200_vec3i *ring, long long ringCap, long long *snapStart,
+                                int *snapCount, int slot, DevCounters *ctr) {
+  const long long ringStart = ctr->ringHead;
+  for (int i = threadIdx.x; i < n; i += blockDim.x) ring[(ringStart + i) % ringCap] = positions[i];
+  __syncthreads();
+  if (threadIdx.x == 0) publish_snapshot(ctr, snapStart, snapCount, slot, ringStart, n);
+}
+
+void launch_push_snapshot(b200_engine *e, const b200_vec3i *positions, int n, int snapSlot) {
+  k_push_snapshot<<<1, 256, 0, e->stream>>>(positions, n, e->d_ring, e->ringCap, e->d_snapStart, e->d_snapCount, snapSlot, e->d_ctr);
+  e->launches++;
+}
+
 static void decay_common(b200_engine *e, const SceneRef &s, int mode, int slot, int minAge, int maxWeight, int frameIdx,
                          long long items) {
   cudaStream_t st = e->stream;

@@ -300,26 +300,46 @@ b200_status b200_reset_scene(b200_engine *e, b200_scene *s) {
   return download_sync(e, s, nullptr);
 }
 
+// Host half of a decay-queue push: the slot the next snapshot goes to, now counted in the queue. The reference's queue of
+// visible-list copies is unbounded (Reco_CUDA.cu:302-317); this one has SNAP_SLOTS frame slots and a ring of list items.
+// When Decay() is never called (--voxel_decay=false) or min_decay_age is very large, the OLDEST snapshot is dropped to make
+// room — never an error (the ring's item overflow is handled the same way on the device: decay.cu recognises an overwritten
+// snapshot by its start position and sweeps nothing).
+static int push_snapshot_slot(b200_engine *e) {
+  if (e->qSize >= SNAP_SLOTS - 1) { e->qHead++; e->qSize--; e->droppedSnapshots++; }
+  const int slot = (e->qHead + e->qSize) % SNAP_SLOTS;
+  e->qSize++;
+  return slot;
+}
+
 static b200_status enqueue_allocate(b200_engine *e, b200_scene *s, b200_render_state *rs, const b200_view *v, int onlyVisible,
                                     bool fuseDeadInit = false) {
-  // The reference's queue of visible-list copies is unbounded (Reco_CUDA.cu:302-317); this one has SNAP_SLOTS frame slots and
-  // a ring of list items. When Decay() is never called (--voxel_decay=false) or min_decay_age is very large, the OLDEST
-  // snapshot is dropped to make room — never an error (the ring's item overflow is handled the same way on the device:
-  // decay.cu recognises an overwritten snapshot by its start position and sweeps nothing).
-  if (e->qSize >= SNAP_SLOTS - 1) { e->qHead++; e->qSize--; e->droppedSnapshots++; }
   if (v->depth_w != e->img_w || v->depth_h != e->img_h) {
     snprintf(e->err, sizeof(e->err), "view size %dx%d differs from engine %dx%d", v->depth_w, v->depth_h, e->img_w, e->img_h);
     return B200_ERR_INVALID;
   }
-  const int slot = (e->qHead + e->qSize) % SNAP_SLOTS;
+  const int slot = push_snapshot_slot(e);
   e->tableVersion++;
   launch_allocate(e, scene_ref(s, rs), frame_geom(s, v), v->d_depth, onlyVisible != 0, e->frameIdx, slot,
                   fuseDeadInit ? rs->d_minmax : nullptr, rs->img_w, rs->img_h);
   e->ptrListFor = rs->d_visibleBlockPositions; e->ptrListVersion = e->tableVersion;
-  e->qSize++;
   e->frameIdx++;
   return B200_OK;
 }
+
+b200_status b200_diag_push_decay_snapshot(b200_engine *e, const b200_vec3i *d_positions, int n) {
+  if (n < 0 || n > e->numBlocks || (n > 0 && !d_positions)) {
+    snprintf(e->err, sizeof(e->err), "a decay snapshot holds 0 to numBlocks (%d) positions, got %d", e->numBlocks, n);
+    return B200_ERR_INVALID;
+  }
+  CK(cudaSetDevice(e->device));
+  launch_push_snapshot(e, d_positions, n, push_snapshot_slot(e));
+  CK(cudaStreamSynchronize(e->stream));
+  CK(cudaGetLastError());
+  return B200_OK;
+}
+
+void b200_diag_set_frame_index(b200_engine *e, int32_t f) { e->frameIdx = f; }
 
 b200_status b200_allocate_from_depth(b200_engine *e, b200_scene *s, b200_render_state *rs, const b200_view *v, int onlyVisible) {
   b200_status st = check_scene(e, s); if (st) return st;

@@ -109,6 +109,16 @@ struct b200_engine {
 
 #define SNAP_SLOTS 4096
 
+// Device half of a decay-queue push (Reco_CUDA.cu:302-316): the `kept` positions written to the ring from ringStart on
+// become snapshot `slot`, and the ring's cursor moves past them. Allocation's list pass and b200_diag_push_decay_snapshot
+// both publish through here; the host half is push_snapshot_slot (engine.cu).
+DEV void publish_snapshot(DevCounters *ctr, long long *snapStart, int *snapCount, int slot, long long ringStart, int kept) {
+  snapStart[slot] = ringStart;
+  snapCount[slot] = kept;
+  ctr->ringHead = ringStart + kept;
+}
+void launch_push_snapshot(b200_engine *e, const b200_vec3i *positions, int n, int snapSlot);
+
 // launchers (each enqueues on e->stream and bumps e->launches)
 void launch_reset(b200_engine *e, const SceneRef &s);
 void launch_allocate(b200_engine *e, const SceneRef &s, const FrameGeom &g, const float *depth, bool onlyVisible,

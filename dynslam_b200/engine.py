@@ -228,6 +228,18 @@ class Engine:
         self.lib.b200_diag_last_integrate(self.h, C.byref(k), C.byref(g))
         return k.value, g.value
 
+    def push_decay_snapshot(self, positions):
+        """test hook (include/b200fusion_diag.h): append a snapshot of block positions (int32 (n, 3) tensor on the engine's
+        device) to the decay queue, as an allocation does, without advancing the frame index"""
+        positions = positions.to(device=self.scene.device, dtype=torch.int32).contiguous()
+        self.after_torch()
+        self.check(self.lib.b200_diag_push_decay_snapshot(self.h, _ptr(positions) if positions.numel() else None,
+                                                          positions.shape[0]))
+
+    def set_frame_index(self, f):
+        """test hook (include/b200fusion_diag.h): the frame index Decay measures block ages against"""
+        self.lib.b200_diag_set_frame_index(self.h, int(f))
+
     # ---- fused fast path --------------------------------------------------------------------
     def process_frame_async(self, renderState, view, points=None, normals=None, decay=None, raycast=True, colour_out=None,
                             depth_out=None):

@@ -47,6 +47,13 @@ void b200_diag_set_max_rendering_blocks(b200_engine *e, int n);
    -1 and 0 before the first launch. Tests use it to check that the variant they mean to exercise really ran. */
 void b200_diag_last_integrate(const b200_engine *e, int *kernel, int *grid);
 
+/* Seed the decay queue the way AllocateSceneFromDepth does (Reco_CUDA.cu:302-316), without an allocation: the n block
+   positions at d_positions (device memory, 0 <= n <= numBlocks) become the newest snapshot, through the same snapshot ring
+   and queue bookkeeping. frameIdx is not advanced; b200_diag_set_frame_index sets it (the `currentFrame` that Decay
+   measures block ages against). Tests use both to hand the engine exactly the decay state they hand the oracle. */
+b200_status b200_diag_push_decay_snapshot(b200_engine *e, const b200_vec3i *d_positions, int n);
+void b200_diag_set_frame_index(b200_engine *e, int32_t f);
+
 /* While the launch trace is on (b200_set_timing(e, 3)) a few CTAs of the allocation's list pass stamp %globaltimer at their
    phase boundaries (8 stamps x 4 CTAs, nanoseconds); copies up to 64 of them out. Measurement only. */
 int b200_diag_read_debug(b200_engine *e, unsigned long long *out, int n);

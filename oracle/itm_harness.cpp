@@ -198,6 +198,89 @@ void harness_download(Harness *H, void *hashOut, void *voxelsOut, void *rayOut, 
   if (imgOut) ORcudaSafeCall(cudaMemcpy(imgOut, H->renderState->raycastImage->GetData(MEMORYDEVICE_CUDA), n * 4, cudaMemcpyDeviceToHost));
 }
 
+void harness_download_lists(Harness *H, int *allocationList, int *excessList, unsigned char *visType) {
+  ORcudaSafeCall(cudaDeviceSynchronize());
+  if (allocationList) ORcudaSafeCall(cudaMemcpy(allocationList, H->scene->localVBA.GetAllocationList(), sizeof(int) * (size_t)H->settings->sdfLocalBlockNum, cudaMemcpyDeviceToHost));
+  if (excessList) ORcudaSafeCall(cudaMemcpy(excessList, H->scene->index.GetExcessAllocationList(), sizeof(int) * (size_t)SDF_EXCESS_LIST_SIZE, cudaMemcpyDeviceToHost));
+  if (visType) ORcudaSafeCall(cudaMemcpy(visType, ((ITMRenderState_VH *)H->renderState)->GetEntriesVisibleType(), (size_t)ITMVoxelBlockHash::noTotalEntries, cudaMemcpyDeviceToHost));
+}
+
+// ---- the reference's own Decay on a state the caller supplies (impl 0 only) ----
+// The reference's allocation is nondeterministic, so a test cannot let it build its own map and compare: it hands the
+// reference exactly the state the oracle decays. The decay queue (frameVisibleBlocks) and the frame index are private
+// members of ITMSceneReconstructionEngine_CUDA. They are reached with pointers-to-member formed in explicit template
+// instantiations, where C++ does not check access ([temp.explicit]/12 of C++14): the reference's headers are included
+// unmodified.
+}  // extern "C"
+typedef ITMSceneReconstructionEngine_CUDA<ITMVoxel, ITMVoxelBlockHash> RefReco;
+template <class Tag, typename Tag::type Member> struct ExposeMember { friend typename Tag::type member(Tag) { return Member; } };
+struct DecayQueueOf { typedef std::queue<VisibleBlockInfo> RefReco::*type; friend type member(DecayQueueOf); };
+struct FrameIdxOf { typedef size_t RefReco::*type; friend type member(FrameIdxOf); };
+template struct ExposeMember<DecayQueueOf, &RefReco::frameVisibleBlocks>;
+template struct ExposeMember<FrameIdxOf, &RefReco::frameIdx>;
+extern "C" {
+
+static RefReco *ref_reco(Harness *H) {
+  if (H->impl != 0) { snprintf(H->err, sizeof(H->err), "the decay entry points drive the reference engine (impl 0) only"); return nullptr; }
+  return static_cast<RefReco *>(H->reco);
+}
+
+// ResetScene (empties the decay queue and the decayed-block count, keeps frameIdx; Reco_CUDA.cu:145-172), then the caller's
+// hash table, voxel block array, allocation list, excess list and visibility bytes, and the two free-list cursors. Decay
+// copies localVBA.lastFreeBlockId to the device itself (:516-519).
+int harness_upload_state(Harness *H, const void *hash, const void *voxels, const int *allocationList, const int *excessList,
+                         const unsigned char *visType, int lastFreeBlockId, int lastFreeExcessListId) {
+  RefReco *reco = ref_reco(H);
+  if (!reco) return 1;
+  reco->ResetScene(H->scene);
+  ORcudaSafeCall(cudaMemcpy(H->scene->index.GetEntries(), hash, sizeof(ITMHashEntry) * (size_t)ITMVoxelBlockHash::noTotalEntries, cudaMemcpyHostToDevice));
+  ORcudaSafeCall(cudaMemcpy(H->scene->localVBA.GetVoxelBlocks(), voxels, sizeof(ITMVoxel) * (size_t)H->scene->localVBA.allocatedSize, cudaMemcpyHostToDevice));
+  ORcudaSafeCall(cudaMemcpy(H->scene->localVBA.GetAllocationList(), allocationList, sizeof(int) * (size_t)H->settings->sdfLocalBlockNum, cudaMemcpyHostToDevice));
+  ORcudaSafeCall(cudaMemcpy(H->scene->index.GetExcessAllocationList(), excessList, sizeof(int) * (size_t)SDF_EXCESS_LIST_SIZE, cudaMemcpyHostToDevice));
+  ORcudaSafeCall(cudaMemcpy(((ITMRenderState_VH *)H->renderState)->GetEntriesVisibleType(), visType, (size_t)ITMVoxelBlockHash::noTotalEntries, cudaMemcpyHostToDevice));
+  H->scene->localVBA.lastFreeBlockId = lastFreeBlockId;
+  H->scene->index.SetLastFreeExcessListId(lastFreeExcessListId);
+  return 0;
+}
+
+// frameVisibleBlocks.push({count, frameIdx, device copy of the positions}), as AllocateSceneFromDepth does (:302-316),
+// including its null block for an empty list
+int harness_push_snapshot(Harness *H, const int *positions, long n) {
+  RefReco *reco = ref_reco(H);
+  if (!reco) return 1;
+  ORUtils::MemoryBlock<Vector3i> *copy = nullptr;
+  if (n > 0) {
+    copy = new ORUtils::MemoryBlock<Vector3i>((size_t)n, MEMORYDEVICE_CUDA);
+    ORcudaSafeCall(cudaMemcpy(copy->GetData(MEMORYDEVICE_CUDA), positions, sizeof(Vector3i) * (size_t)n, cudaMemcpyHostToDevice));
+  }
+  const size_t f = reco->*member(FrameIdxOf());
+  (reco->*member(DecayQueueOf())).push(VisibleBlockInfo{(size_t)n, f, copy});
+  return 0;
+}
+
+int harness_set_frame_index(Harness *H, long f) {
+  RefReco *reco = ref_reco(H);
+  if (!reco) return 1;
+  reco->*member(FrameIdxOf()) = (size_t)f;
+  return 0;
+}
+
+long harness_queue_size(Harness *H) {
+  RefReco *reco = ref_reco(H);
+  return reco ? (long)(reco->*member(DecayQueueOf())).size() : -1;
+}
+
+// the reference's own ITMSceneReconstructionEngine_CUDA::Decay (host method and kernels, :509-560); *decayed receives
+// GetDecayedBlockCount() (blocks freed since the upload's ResetScene)
+int harness_decay(Harness *H, int maxWeight, int minAge, int forceAll, long *decayed) {
+  RefReco *reco = ref_reco(H);
+  if (!reco) return 1;
+  reco->Decay(H->scene, H->renderState, maxWeight, minAge, forceAll != 0);
+  ORcudaSafeCall(cudaDeviceSynchronize());
+  *decayed = (long)reco->GetDecayedBlockCount();
+  return 0;
+}
+
 // ---- view builder (SURVEY 8(f) rank 1): ITMViewBuilder_CUDA (impl 0) vs ITMViewBuilder_B200 (impl 1) ----
 struct VBHarness {
   int impl;

@@ -172,6 +172,28 @@ void oracle_engine_destroy(oracle_engine *e) {
   free(e->allocType); free(e->blockCoords); free(e->allocatedBlockPositions); free(e);
 }
 
+/* frameVisibleBlocks.push({count, frameIdx, copy of the positions}) — CUDA/..._CUDA.cu:302-316. Allocation pushes its
+   visible list here; tests push a snapshot of their own to seed the decay queue. */
+void oracle_push_snapshot(oracle_engine *e, const b200_vec3i *positions, int n) {
+  snap *sn = (snap *)calloc(1, sizeof(snap));
+  sn->count = n; sn->frameIdx = e->frameIdx;
+  if (n > 0) {
+    sn->items = (b200_vec3i *)malloc(sizeof(b200_vec3i) * (size_t)n);
+    memcpy(sn->items, positions, sizeof(b200_vec3i) * (size_t)n);
+  }
+  if (e->q_tail) e->q_tail->next = sn; else e->q_head = sn;
+  e->q_tail = sn; e->q_size++;
+}
+
+/* the front (oldest) snapshot: copies up to cap positions to out, returns its count, or -1 when the queue is empty */
+int oracle_peek_snapshot(const oracle_engine *e, b200_vec3i *out, int cap) {
+  if (!e->q_head) return -1;
+  const int n = e->q_head->count;
+  if (out && n > 0) memcpy(out, e->q_head->items, sizeof(b200_vec3i) * (size_t)(n < cap ? n : cap));
+  return n;
+}
+
+void oracle_set_frame_index(oracle_engine *e, int f) { e->frameIdx = f; }
 int oracle_frame_index(const oracle_engine *e) { return e->frameIdx; }
 long oracle_decayed_block_count(const oracle_engine *e) { return e->totalDecayed; }
 int oracle_queue_size(const oracle_engine *e) { return e->q_size; }
@@ -387,14 +409,7 @@ int oracle_allocate_from_depth(oracle_engine *e, b200_scene *s, b200_render_stat
   s->lastFreeExcessListId = lastFreeExcessListId;
 
   /* decay queue snapshot + frameIdx++ — :302-317 */
-  snap *sn = (snap *)calloc(1, sizeof(snap));
-  sn->count = noVisible; sn->frameIdx = e->frameIdx;
-  if (noVisible > 0) {
-    sn->items = (b200_vec3i *)malloc(sizeof(b200_vec3i) * (size_t)noVisible);
-    memcpy(sn->items, rs->d_visibleBlockPositions, sizeof(b200_vec3i) * (size_t)noVisible);
-  }
-  if (e->q_tail) e->q_tail->next = sn; else e->q_head = sn;
-  e->q_tail = sn; e->q_size++;
+  oracle_push_snapshot(e, rs->d_visibleBlockPositions, noVisible);
   e->frameIdx++;
 
   if (s->lastFreeBlockId < 0) return B200_ERR_VBA_FULL;
@@ -524,6 +539,18 @@ void oracle_integrate(oracle_engine *e, b200_scene *s, const b200_render_state *
 /* Decay — CUDA/..._CUDA.cu:509-560; decayVoxel :1120-1197; deleteBlock :1012-1115 (serial: the     */
 /* bucket lock never contends). Blocks in list order (partial) / ascending VBA id (full).        */
 /* ------------------------------------------------------------------------------------------- */
+/* How often each decay branch ran since the last oracle_decay_branches() call: tests use it to check that the branch they
+   target really ran. */
+enum { DB_AGE_SKIP, DB_VOXEL_RESET, DB_HEAD_WITH_SUCCESSOR, DB_HEAD_ALONE, DB_EXCESS_ENTRY, DB_COUNT };
+static long g_decay_branch[DB_COUNT];
+
+/* copies the counters {blocks left alone because age < minAge, voxels reset, deleted bucket heads with a successor, deleted
+   bucket heads without one, deleted excess-list entries} to out and clears them */
+void oracle_decay_branches(long *out) {
+  memcpy(out, g_decay_branch, sizeof(g_decay_branch));
+  memset(g_decay_branch, 0, sizeof(g_decay_branch));
+}
+
 static void delete_block(b200_scene *s, uint8_t *visType, int x, int y, int z, int *lastFree) {
   b200_hash_entry *table = s->d_hash; const int nb = s->numBuckets;
   int prev;
@@ -531,6 +558,7 @@ static void delete_block(b200_scene *s, uint8_t *visType, int x, int y, int z, i
   if (idx < 0) return; /* cannot happen in the serial order; the reference would index -1 here */
   int freeListIdx = (*lastFree)++;
   s->d_allocationList[freeListIdx + 1] = table[idx].ptr;
+  g_decay_branch[prev != -1 ? DB_EXCESS_ENTRY : (table[idx].offset >= 1 ? DB_HEAD_WITH_SUCCESSOR : DB_HEAD_ALONE)]++;
   if (prev == -1) {
     if (table[idx].offset >= 1) {
       int nextIdx = nb + table[idx].offset - 1;
@@ -558,13 +586,14 @@ static void decay_block(b200_scene *s, uint8_t *visType, int x, int y, int z, in
   int idx = find_block_prev(s->d_hash, s->numBuckets, x, y, z, &prev);
   if (idx < 0) return;
   int age = currentFrame - s->d_hash[idx].allocatedTime;
-  if (age < minAge) return; /* safeToClear == false: nothing touched, never deleted (:1151-1157, :1189) */
+  if (age < minAge) { g_decay_branch[DB_AGE_SKIP]++; return; } /* safeToClear == false: nothing touched, never deleted (:1151-1157, :1189) */
   b200_voxel *blk = &s->d_voxels[(size_t)s->d_hash[idx].ptr * BS3];
   int empty = 0;
   for (int i = 0; i < BS3; ++i) {
     int isNoisy = (blk[i].w_depth <= maxWeight);
     if (isNoisy && blk[i].w_depth > 0) {
       blk[i].sdf = 32767; blk[i].w_depth = 0; blk[i].clr[0] = blk[i].clr[1] = blk[i].clr[2] = 0; blk[i].w_color = 0;
+      g_decay_branch[DB_VOXEL_RESET]++;
     }
     if (blk[i].w_depth == 0) empty++;
   }

@@ -17,6 +17,18 @@ def available():
     return os.path.exists(SO)
 
 
+# Entry points that run the reference's own Decay on a supplied state. Where the reference's sources cannot be read at
+# build time, oracle/build_ref.sh keeps an oracle/_ref built earlier, which may predate them: the other harness tests
+# still run against such a library, and the decay tests run without the reference (its outcomes stay pinned in
+# tests/golden/ref_pins.json).
+DECAY_ENTRY_POINTS = ("harness_upload_state", "harness_push_snapshot", "harness_set_frame_index", "harness_queue_size",
+                      "harness_decay", "harness_download_lists")
+
+
+def decay_available():
+    return available() and all(hasattr(lib(), n) for n in DECAY_ENTRY_POINTS)
+
+
 _L = None
 
 
@@ -45,6 +57,15 @@ def lib():
         L.harness_counters.restype = None
         L.harness_download.argtypes = [vp, vp, vp, vp, vp]
         L.harness_download.restype = None
+        if all(hasattr(L, n) for n in DECAY_ENTRY_POINTS):
+            L.harness_download_lists.argtypes = [vp, vp, vp, vp]
+            L.harness_download_lists.restype = None
+            L.harness_upload_state.argtypes = [vp, vp, vp, vp, vp, vp, C.c_int, C.c_int]
+            L.harness_push_snapshot.argtypes = [vp, vp, C.c_long]
+            L.harness_set_frame_index.argtypes = [vp, C.c_long]
+            L.harness_queue_size.argtypes = [vp]
+            L.harness_queue_size.restype = C.c_long
+            L.harness_decay.argtypes = [vp, C.c_int, C.c_int, C.c_int, C.POINTER(C.c_long)]
         L.vbh_create.restype = vp
         L.vbh_create.argtypes = [C.c_int, C.c_int, C.c_int, C.c_float, C.c_float, C.c_float, C.c_float]
         L.vbh_destroy.argtypes = [vp]
@@ -131,6 +152,43 @@ class Harness:
         img = np.zeros((self.h, self.w, 4), dtype=np.uint8)
         self.L.harness_download(self.h_, hash_.ctypes.data, vox.ctypes.data, rays.ctypes.data, img.ctypes.data)
         return dict(hash=hash_, voxels=vox, rays=rays, image=img)
+
+    # ---- the reference's own Decay on a supplied state (REFERENCE_CUDA only) ----
+    def _ok(self, rc):
+        if rc:
+            raise RuntimeError(self.L.harness_error(self.h_).decode())
+
+    def upload_state(self, hash_, voxels, allocationList, excessList, visType, lastFreeBlockId, lastFreeExcessListId):
+        """ResetScene (empties the decay queue, keeps the frame index), then the given state"""
+        arrs = [np.ascontiguousarray(a) for a in (hash_, voxels, allocationList, excessList, visType)]
+        assert arrs[0].nbytes == self.noTotal * 20 and arrs[1].nbytes == self.numBlocks * 512 * 8 and arrs[4].nbytes == self.noTotal
+        self._ok(self.L.harness_upload_state(self.h_, *[a.ctypes.data for a in arrs], int(lastFreeBlockId), int(lastFreeExcessListId)))
+
+    def push_snapshot(self, positions):
+        p = np.ascontiguousarray(positions, dtype=np.int32).reshape(-1, 3)
+        self._ok(self.L.harness_push_snapshot(self.h_, p.ctypes.data if len(p) else None, len(p)))
+
+    def set_frame_index(self, f):
+        self._ok(self.L.harness_set_frame_index(self.h_, int(f)))
+
+    def queue_size(self):
+        return self.L.harness_queue_size(self.h_)
+
+    def decay(self, maxWeight, minAge, forceAll=False):
+        """the reference's Decay; returns GetDecayedBlockCount() (blocks freed since the last upload_state)"""
+        n = C.c_long()
+        self._ok(self.L.harness_decay(self.h_, int(maxWeight), int(minAge), int(forceAll), C.byref(n)))
+        return n.value
+
+    def download_state(self, excessSize):
+        d = self.download()
+        alloc = np.zeros(self.numBlocks, np.int32)
+        exl = np.zeros(excessSize, np.int32)
+        vis = np.zeros(self.noTotal, np.uint8)
+        self.L.harness_download_lists(self.h_, alloc.ctypes.data, exl.ctypes.data, vis.ctypes.data)
+        c = self.counters()
+        return dict(hash=d["hash"], voxels=d["voxels"], allocationList=alloc, excessList=exl, visType=vis,
+                    lastFreeBlockId=c["lastFreeBlockId"], lastFreeExcessListId=c["lastFreeExcessListId"])
 
     def close(self):
         if self.h_:

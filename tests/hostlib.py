@@ -53,6 +53,13 @@ def oracle():
     L.oracle_integrate.argtypes = [vp, P(abi.Scene), P(abi.RenderState), P(abi.View), C.c_int]
     L.oracle_integrate.restype = None
     L.oracle_decay.argtypes = [vp, P(abi.Scene), P(abi.RenderState), C.c_int, C.c_int, C.c_int]
+    L.oracle_push_snapshot.argtypes = [vp, vp, C.c_int]
+    L.oracle_push_snapshot.restype = None
+    L.oracle_peek_snapshot.argtypes = [vp, vp, C.c_int]
+    L.oracle_set_frame_index.argtypes = [vp, C.c_int]
+    L.oracle_set_frame_index.restype = None
+    L.oracle_decay_branches.argtypes = [P(C.c_long)]
+    L.oracle_decay_branches.restype = None
     L.oracle_find_visible_blocks.argtypes = [P(abi.Scene), P(abi.RenderState), P(abi.Camera)]
     L.oracle_find_visible_blocks.restype = None
     L.oracle_expected_depths.argtypes = [P(abi.Scene), P(abi.RenderState), P(abi.Camera)]

@@ -8,6 +8,8 @@ differs. Where oracle/_ref is built, the test also runs the reference itself and
 
 After a deliberate change of a pinned test's inputs, record the digests again where oracle/_ref is built:
     REFPINS_RECORD=1 python -m pytest tests/test_oracle_vs_ref.py tests/test_eval_oracle.py tests/test_frames_oracle.py tests/test_hostio.py
+The decay pins need the reference's CUDA Decay, so they are recorded on the GPU:
+    REFPINS_RECORD=1 python -m pytest tests/test_gpu_decay.py
 """
 import atexit
 import hashlib

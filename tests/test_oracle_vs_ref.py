@@ -9,7 +9,7 @@ import pytest
 
 from dynslam_b200 import abi, synth
 from tests import hostlib as H
-from tests import refpins
+from tests import decaylib, refpins
 
 
 def _ref_or_none():
@@ -384,3 +384,14 @@ def test_mesh_oracle_equals_reference_cpu_engine():
     refpins.check("oracle_vs_ref/mesh_scene", np.int64(na).tobytes() + a[:na].tobytes(), ref)
     # colours are really interpolated from the volume, vertices lie inside the fused region
     assert a["c0"][:na].max() > 0.2 and np.isfinite(a["p0"][:na]).all()
+
+
+@pytest.mark.parametrize("name", list(decaylib.pinned_cases()))
+def test_decay_pinned_to_reference(name):
+    """The oracle's Decay (oracle_decay, delete_block, decay_block) against the reference's own CUDA Decay
+    (ITMSceneReconstructionEngine_CUDA.cu:509-560, :1012-1262) on the crafted, street and queue cases of tests/decaylib.py:
+    hash table, visibility bytes, the allocation list with each freed section sorted (the reference pushes freed blocks with
+    atomicAdd), the free-list cursors, the decayed count and the voxel block array. The reference's decay is CUDA-only, so
+    its outcomes were recorded on an H100 by tests/test_gpu_decay.py, which also runs it live."""
+    o = decaylib.run_oracle(*decaylib.pinned_cases()[name]())
+    refpins.check(decaylib.pin_key(name), decaylib.outcome_bytes(o.calls[-1]["post"], decaylib.sections_of(o), o.calls[-1]["decayed"]))
