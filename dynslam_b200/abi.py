@@ -119,6 +119,15 @@ class ViewCalib(C.Structure):
                 ("intrinsics_d", C.c_float * 4), ("useBilateralFilter", C.c_int32), ("modelSensorNoise", C.c_int32)]
 
 
+class DepthInput(C.Structure):
+    """b200_depth_input: which stored depth a stereo-input frame carries, the stereo rig and DepthProvider's depth bounds."""
+    _fields_ = [("kind", C.c_int32), ("baseline_m", C.c_float), ("focal_length_px", C.c_float), ("min_depth_m", C.c_float),
+                ("max_depth_m", C.c_float)]
+
+
+DEPTH_IN_DISPARITY_F32, DEPTH_IN_DEPTH_MM_S16 = 0, 1
+
+
 class Mask(C.Structure):
     """b200_mask: inclusive bounding box + box-sized u8 mask (1 = inside)."""
     _fields_ = [("x0", C.c_int32), ("y0", C.c_int32), ("x1", C.c_int32), ("y1", C.c_int32), ("d_data", C.c_void_p)]
@@ -152,6 +161,7 @@ EXPORTS = [
     "b200_process_frame_host", "b200_host_frame_submit", "b200_host_frame_wait",
     "b200_convert_disparity_to_depth", "b200_convert_depth_affine_to_float", "b200_depth_filtering",
     "b200_compute_normal_and_weights", "b200_update_view", "b200_update_view_async", "b200_host_frame_submit_raw",
+    "b200_depth_mm_from_input", "b200_bgr_to_rgba", "b200_host_frame_submit_stereo",
     "b200_process_silhouettes", "b200_process_silhouettes_async", "b200_composite_depth", "b200_composite_color",
     "b200_composite_instances", "b200_evaluate_depth",
     "b200_mesh_scene", "b200_comm_unique_id", "b200_comm_create", "b200_comm_destroy", "b200_comm_last_error", "b200_gather_composite_submit",
@@ -215,6 +225,10 @@ def load_library():
     lib.b200_update_view_async.argtypes = [vp, vp, C.c_int, C.c_int, P(ViewCalib), vp, vp, vp]
     lib.b200_host_frame_submit_raw.argtypes = [vp, P(Scene), P(RenderState), P(View), vp, vp, P(ViewCalib), vp, vp, P(FrameOpts),
                                                vp, C.c_int]
+    lib.b200_depth_mm_from_input.argtypes = [vp, vp, vp, C.c_int, C.c_int, P(DepthInput)]
+    lib.b200_bgr_to_rgba.argtypes = [vp, vp, vp, C.c_int, C.c_int]
+    lib.b200_host_frame_submit_stereo.argtypes = [vp, P(Scene), P(RenderState), P(View), vp, vp, P(DepthInput), P(ViewCalib), vp, vp,
+                                                  P(FrameOpts), vp, vp, C.c_int]
     lib.b200_process_silhouettes.argtypes = [vp, vp, vp, C.c_int, C.c_int, P(SilhouetteOp), C.c_int]
     lib.b200_process_silhouettes_async.argtypes = [vp, vp, vp, C.c_int, C.c_int, P(SilhouetteOp), C.c_int]
     lib.b200_composite_depth.argtypes = [vp, vp, vp, C.c_int]

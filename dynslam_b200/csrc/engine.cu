@@ -12,6 +12,7 @@
 #include "engine.h"
 #include "../../include/b200fusion_diag.h"
 
+#include <cmath>
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
@@ -216,7 +217,7 @@ void b200_engine_destroy(b200_engine *e) {
   for (int i = 0; i < 8; ++i) if (e->ev[i]) cudaEventDestroy(e->ev[i]);
   if (e->copyStream) {
     cudaStreamSynchronize(e->copyStream);
-    for (int i = 0; i < 2; ++i) { cudaFree(e->d_stageDepth[i]); cudaFree(e->d_stageRgb[i]); cudaFree(e->d_stageOut[i]); cudaFree(e->d_stageRaw[i]);
+    for (int i = 0; i < 2; ++i) { cudaFree(e->d_stageDepth[i]); cudaFree(e->d_stageRgb[i]); cudaFree(e->d_stageOut[i]); cudaFree(e->d_stageRaw[i]); cudaFree(e->d_stageBgr[i]);
       if (e->evH2D[i]) cudaEventDestroy(e->evH2D[i]); if (e->evCompute[i]) cudaEventDestroy(e->evCompute[i]); if (e->evD2H[i]) cudaEventDestroy(e->evD2H[i]); }
     cudaStreamDestroy(e->copyStream);
     if (e->d2hStream) { cudaStreamSynchronize(e->d2hStream); cudaStreamDestroy(e->d2hStream); }
@@ -689,9 +690,10 @@ static b200_status ensure_pipeline(b200_engine *e, size_t pixels) {
     }
   }
   for (int i = 0; i < 2; ++i) {
-    cudaFree(e->d_stageDepth[i]); cudaFree(e->d_stageRgb[i]); cudaFree(e->d_stageOut[i]); cudaFree(e->d_stageRaw[i]);
+    cudaFree(e->d_stageDepth[i]); cudaFree(e->d_stageRgb[i]); cudaFree(e->d_stageOut[i]); cudaFree(e->d_stageRaw[i]); cudaFree(e->d_stageBgr[i]);
     CK(cudaMalloc(&e->d_stageDepth[i], pixels * sizeof(float)));
     CK(cudaMalloc(&e->d_stageRaw[i], pixels * sizeof(int16_t)));
+    CK(cudaMalloc(&e->d_stageBgr[i], pixels * 3));
     CK(cudaMalloc(&e->d_stageRgb[i], pixels * sizeof(b200_vec4u)));
     CK(cudaMalloc(&e->d_stageOut[i], pixels * sizeof(b200_vec4u)));
     e->slotBusy[i] = false;
@@ -816,9 +818,15 @@ b200_status b200_composite_color(b200_engine *e, b200_vec4u *d_target_color, flo
 }
 
 // ---- pipelined host frames ----------------------------------------------------------------------------
+// A stereo-input frame (b200_host_frame_submit_stereo): the stored depth and the BGR colour, uploaded and converted on the copy stream.
+struct StereoFrame {
+  const uint8_t *h_bgr; const void *h_depthIn; int kind; float fb; int minMm, maxMm; int16_t *d_depthMmOut;
+};
+
 static b200_status host_frame_submit(b200_engine *e, b200_scene *s, b200_render_state *rs, b200_view *v, const float *h_depth,
                                      const int16_t *h_raw, const b200_view_calib *calib, const b200_vec4u *h_rgb, b200_vec4f *d_points,
-                                     b200_vec4f *d_normals, const b200_frame_opts *opts, b200_vec4u *h_outImage, int slot) {
+                                     b200_vec4f *d_normals, const b200_frame_opts *opts, b200_vec4u *h_outImage, int slot,
+                                     const StereoFrame *stereo = nullptr) {
   if (slot < 0 || slot > 1) { snprintf(e->err, sizeof(e->err), "slot must be 0 or 1"); return B200_ERR_INVALID; }
   CK(cudaSetDevice(e->device));
   const size_t nd = (size_t)v->depth_w * v->depth_h, nc = (size_t)v->rgb_w * v->rgb_h, no = (size_t)rs->img_w * rs->img_h;
@@ -830,14 +838,26 @@ static b200_status host_frame_submit(b200_engine *e, b200_scene *s, b200_render_
   // the latency-bound scan kernels of the allocation stage down by 2x when they overlap; under the raycast it is free.
   if (e->midValid) CK(cudaStreamWaitEvent(e->copyStream, e->evMid, 0));
   trace_begin(e, e->copyStream, "h2d_frame");
-  if (h_raw) CK(cudaMemcpyAsync(e->d_stageRaw[slot], h_raw, nd * sizeof(int16_t), cudaMemcpyHostToDevice, e->copyStream));
+  if (stereo) {
+    // The disparity goes into the slot's float depth image, which UpdateView overwrites only after evH2D; the conversion writes
+    // the int16 image UpdateView reads. Running here, it overlaps the previous frame's kernels as the copies do.
+    if (stereo->kind == B200_DEPTH_IN_DISPARITY_F32) CK(cudaMemcpyAsync(e->d_stageDepth[slot], stereo->h_depthIn, nd * sizeof(float), cudaMemcpyHostToDevice, e->copyStream));
+    else CK(cudaMemcpyAsync(e->d_stageRaw[slot], stereo->h_depthIn, nd * sizeof(int16_t), cudaMemcpyHostToDevice, e->copyStream));
+    CK(cudaMemcpyAsync(e->d_stageBgr[slot], stereo->h_bgr, nc * 3, cudaMemcpyHostToDevice, e->copyStream));
+  } else if (h_raw) CK(cudaMemcpyAsync(e->d_stageRaw[slot], h_raw, nd * sizeof(int16_t), cudaMemcpyHostToDevice, e->copyStream));
   else CK(cudaMemcpyAsync(e->d_stageDepth[slot], h_depth, nd * sizeof(float), cudaMemcpyHostToDevice, e->copyStream));
-  CK(cudaMemcpyAsync(e->d_stageRgb[slot], h_rgb, nc * sizeof(b200_vec4u), cudaMemcpyHostToDevice, e->copyStream));
+  if (!stereo) CK(cudaMemcpyAsync(e->d_stageRgb[slot], h_rgb, nc * sizeof(b200_vec4u), cudaMemcpyHostToDevice, e->copyStream));
   trace_end(e, e->copyStream);
+  if (stereo) {
+    const void *in = stereo->kind == B200_DEPTH_IN_DISPARITY_F32 ? (const void *)e->d_stageDepth[slot] : (const void *)e->d_stageRaw[slot];
+    launch_stereo_input(e, e->copyStream, in, stereo->kind, (int)nd, stereo->fb, stereo->minMm, stereo->maxMm, e->d_stageRaw[slot],
+                        stereo->d_depthMmOut, e->d_stageBgr[slot], e->d_stageRgb[slot], (int)nc);
+    CK(cudaGetLastError());
+  }
   CK(cudaEventRecord(e->evH2D[slot], e->copyStream));
   // the frame on the compute stream
   CK(cudaStreamWaitEvent(e->stream, e->evH2D[slot], 0));
-  if (h_raw) {
+  if (h_raw || stereo) {
     st = b200_update_view_async(e, e->d_stageRaw[slot], v->depth_w, v->depth_h, calib, e->d_stageDepth[slot], nullptr, nullptr);
     if (st) return st;
   }
@@ -872,6 +892,67 @@ b200_status b200_host_frame_submit_raw(b200_engine *e, b200_scene *s, b200_rende
   if (!h_rawDepth || !calib) { snprintf(e->err, sizeof(e->err), "raw depth / calibration missing"); return B200_ERR_INVALID; }
   if (calib->modelSensorNoise) { snprintf(e->err, sizeof(e->err), "modelSensorNoise is not available on the pipelined path; call b200_update_view"); return B200_ERR_INVALID; }
   return host_frame_submit(e, s, rs, v, nullptr, h_rawDepth, calib, h_rgb, d_points, d_normals, opts, h_outImage, slot);
+}
+
+// DepthFromDisparityMap's bounds (DepthProvider.h:107-117) for kind 0, ReadPrecomputed's (int16_t)round(max * 1000) for kind 1
+// (PrecomputedDepthProvider.cpp:54-55). The reference's casts are undefined outside the target range; they are evaluated with
+// x86's convention (INT_MIN, then the low 16 bits), so the bounds are the ones the reference's x86 build uses.
+static int32_t x86_trunc_i32(double x) { return (x > -2147483649.0 && x < 2147483648.0) ? (int32_t)x : INT32_MIN; }
+
+static b200_status depth_input_bounds(b200_engine *e, const b200_depth_input *in, float *fb, int *minMm, int *maxMm) {
+  if (!in) { snprintf(e->err, sizeof(e->err), "depth input parameters missing"); return B200_ERR_INVALID; }
+  if (in->kind != B200_DEPTH_IN_DISPARITY_F32 && in->kind != B200_DEPTH_IN_DEPTH_MM_S16) {
+    snprintf(e->err, sizeof(e->err), "unknown depth input kind %d", in->kind); return B200_ERR_INVALID;
+  }
+  const float maxF = in->max_depth_m * 1000.0f;
+  const int32_t max_depth_mm = x86_trunc_i32(maxF);
+  const int32_t max_representable_depth = 32767;   // std::numeric_limits<int16_t>::max()
+  if (max_depth_mm >= max_representable_depth) {    // the reference's text, DepthProvider.h:113-117
+    snprintf(e->err, sizeof(e->err), "Unsupported maximum depth of %f meters (%d mm, larger than the %d limit).", in->max_depth_m,
+             max_depth_mm, max_representable_depth);
+    return B200_ERR_INVALID;
+  }
+  if (in->kind == B200_DEPTH_IN_DISPARITY_F32) {
+    *fb = in->focal_length_px * in->baseline_m;     // PrecomputedDepthProvider::DepthFromDisparity's order
+    *minMm = x86_trunc_i32(in->min_depth_m * 1000.0f);
+    *maxMm = max_depth_mm;
+  } else {
+    *fb = 0.0f; *minMm = INT32_MIN;
+    *maxMm = (int16_t)(uint16_t)(uint32_t)x86_trunc_i32(round((double)maxF));
+  }
+  return B200_OK;
+}
+
+b200_status b200_depth_mm_from_input(b200_engine *e, int16_t *d_out_mm, const void *d_in, int w, int h, const b200_depth_input *in) {
+  b200_status st = check_image(e, d_out_mm, d_in, w, h); if (st) return st;
+  float fb; int minMm, maxMm;
+  st = depth_input_bounds(e, in, &fb, &minMm, &maxMm); if (st) return st;
+  CK(cudaSetDevice(e->device));
+  launch_stereo_input(e, e->stream, d_in, in->kind, w * h, fb, minMm, maxMm, d_out_mm, nullptr, nullptr, nullptr, 0);
+  CK(cudaStreamSynchronize(e->stream)); CK(cudaGetLastError());
+  return B200_OK;
+}
+
+b200_status b200_bgr_to_rgba(b200_engine *e, b200_vec4u *d_out, const uint8_t *d_bgr, int w, int h) {
+  b200_status st = check_image(e, d_out, d_bgr, w, h); if (st) return st;
+  CK(cudaSetDevice(e->device));
+  launch_stereo_input(e, e->stream, nullptr, 0, 0, 0.0f, 0, 0, nullptr, nullptr, d_bgr, d_out, w * h);
+  CK(cudaStreamSynchronize(e->stream)); CK(cudaGetLastError());
+  return B200_OK;
+}
+
+// Input::ReadNextFrame's DepthFromStereo (DS/Input.cpp:41-97) + CvToItm (DS/InfiniTamDriver.cpp:81-100) + UpdateView + the fused frame
+b200_status b200_host_frame_submit_stereo(b200_engine *e, b200_scene *s, b200_render_state *rs, b200_view *v, const uint8_t *h_bgr,
+                                          const void *h_depthIn, const b200_depth_input *in, const b200_view_calib *calib,
+                                          b200_vec4f *d_points, b200_vec4f *d_normals, const b200_frame_opts *opts, b200_vec4u *h_outImage,
+                                          int16_t *d_depthMmOut, int slot) {
+  if (!h_bgr || !h_depthIn || !calib) { snprintf(e->err, sizeof(e->err), "stereo input: colour, depth input or calibration missing"); return B200_ERR_INVALID; }
+  if (v->depth_w < 5 || v->depth_h < 5 || v->rgb_w < 5 || v->rgb_h < 5) { snprintf(e->err, sizeof(e->err), "stereo input: image smaller than 5x5"); return B200_ERR_INVALID; }
+  if (calib->modelSensorNoise) { snprintf(e->err, sizeof(e->err), "modelSensorNoise is not available on the pipelined path; call b200_update_view"); return B200_ERR_INVALID; }
+  StereoFrame sf{h_bgr, h_depthIn, 0, 0.0f, 0, 0, d_depthMmOut};
+  b200_status st = depth_input_bounds(e, in, &sf.fb, &sf.minMm, &sf.maxMm); if (st) return st;
+  sf.kind = in->kind;
+  return host_frame_submit(e, s, rs, v, nullptr, nullptr, calib, nullptr, d_points, d_normals, opts, h_outImage, slot, &sf);
 }
 
 b200_status b200_host_frame_wait(b200_engine *e, int slot) {

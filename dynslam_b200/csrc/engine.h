@@ -76,6 +76,7 @@ struct b200_engine {
   cudaStream_t copyStream;     // H2D of the next frame's depth + RGB
   cudaStream_t d2hStream;      // D2H of the previous frame's image (own stream so it never holds up the next upload)
   float *d_stageDepth[2]; b200_vec4u *d_stageRgb[2]; b200_vec4u *d_stageOut[2]; int16_t *d_stageRaw[2];
+  uint8_t *d_stageBgr[2];      // BGR8 colour of a stereo-input frame (b200_host_frame_submit_stereo), 3 B/px
   cudaEvent_t evH2D[2], evCompute[2], evD2H[2];
   bool slotBusy[2]; size_t stagePixels;
   int maxRenderingBlocks;                           // MAX_RENDERING_BLOCKS; b200_diag_set_max_rendering_blocks lowers it (tests)
@@ -162,6 +163,10 @@ void launch_view_filter_pass(b200_engine *e, const float *in, float *out, int w,
 void launch_update_view(b200_engine *e, const int16_t *raw, float *out, float *scratch, int w, int h, int type, float p0, float p1,
                         float fx, bool filter);
 void launch_view_normals(b200_engine *e, const float *depth, b200_vec4f *normal, float *sigmaZ, int w, int h, const float intr[4]);
+// input.cu: int16 mm depth from a disparity map (kind 0) or a clamped int16 depth map (kind 1), and BGR8 -> RGBA8, on stream st.
+// depthOut / rgba may be null (that half is skipped); depthCopy (may be null) receives a second copy of the depth.
+void launch_stereo_input(b200_engine *e, cudaStream_t st, const void *depthIn, int kind, int nDepth, float fb, int minMm, int maxMm,
+                         int16_t *depthOut, int16_t *depthCopy, const uint8_t *bgr, b200_vec4u *rgba, int nColour);
 
 void launch_process_silhouettes(b200_engine *e, b200_vec4u *rgb, float *depth, int w, int h, const b200_silhouette_op *ops, int n);
 void launch_composite_depth(b200_engine *e, float *target, const float *source, int n);

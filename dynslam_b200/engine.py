@@ -290,6 +290,20 @@ class Engine:
                                                         _ptr(h_raw), _ptr(h_rgb), C.byref(calib), _ptr(points), _ptr(normals),
                                                         C.byref(o), _ptr(h_out), slot))
 
+    def host_frame_submit_stereo(self, renderState, view, h_bgr, h_depth_in, depth_input, calib, points=None, normals=None, decay=None,
+                                 raycast=True, h_out=None, depth_mm_out=None, slot=0):
+        """As host_frame_submit_raw, from DynSLAM's stored stereo input: h_bgr (h, w, 3 uint8, OpenCV's BGR) and h_depth_in (a float32
+        disparity map or int16 millimetres, per depth_input.kind; see make_depth_input). The int16 mm depth and the RGBA colour are
+        made on the device; depth_mm_out (an int16 CUDA tensor, optional) receives the frame's int16 mm depth once
+        host_frame_wait(slot) returns."""
+        o = abi.FrameOpts()
+        o.doRaycast = int(raycast)
+        if decay is not None:
+            o.doDecay, o.decayMaxWeight, o.decayMinAge = 1, decay[0], decay[1]
+        self.check(self.lib.b200_host_frame_submit_stereo(self.h, C.byref(self.scene.c), C.byref(renderState.c), C.byref(view.c),
+                                                           _ptr(h_bgr), _ptr(h_depth_in), C.byref(depth_input), C.byref(calib),
+                                                           _ptr(points), _ptr(normals), C.byref(o), _ptr(h_out), _ptr(depth_mm_out), slot))
+
     def trace(self):
         """Launch trace collected since set_timing(3): list of (kernel, start_us, end_us)."""
         buf = C.create_string_buffer(1 << 20)
@@ -315,6 +329,35 @@ def make_view_calib(trafoType=1, params=(1.0 / 1000.0, 0.0), fx_depth=0.0, intri
     c.intrinsics_d = (C.c_float * 4)(*[float(x) for x in intrinsics_d])
     c.useBilateralFilter, c.modelSensorNoise = int(useBilateralFilter), int(modelSensorNoise)
     return c
+
+
+def make_depth_input(kind=abi.DEPTH_IN_DISPARITY_F32, baseline_m=0.0, focal_length_px=0.0, min_depth_m=0.5, max_depth_m=20.0):
+    """b200_depth_input. kind 0: a DispNet float disparity map with the rig's StereoCalibration (DS/DepthProvider.h:22-28);
+    kind 1: an ELAS int16 millimetre depth map. min/max: DepthProvider's depth bounds (the KITTI configurations' 0.5 m and 20 m, DS/Input.h:71-72)."""
+    d = abi.DepthInput()
+    d.kind, d.baseline_m, d.focal_length_px = int(kind), float(baseline_m), float(focal_length_px)
+    d.min_depth_m, d.max_depth_m = float(min_depth_m), float(max_depth_m)
+    return d
+
+
+class StereoInput:
+    """DynSLAM's per-frame input conversions on the device (images are torch CUDA tensors), named after the reference's functions."""
+
+    def __init__(self, engine, depth_input):
+        self.e, self.depth_input = engine, depth_input
+
+    def DepthFromDisparityMap(self, out_depth, disparity):
+        """DepthProvider::DepthFromDisparityMap<float> with scale 1 (kind 0), or ReadPrecomputed's max-depth clamp of a stored int16
+        depth map (kind 1; out_depth may be the input): int16 millimetres into out_depth."""
+        ViewBuilder._inputs_ready()
+        h, w = disparity.shape
+        self.e.check(self.e.lib.b200_depth_mm_from_input(self.e.h, _ptr(out_depth), _ptr(disparity), w, h, C.byref(self.depth_input)))
+
+    def CvToItm(self, out_rgba, bgr):
+        """CvToItm(const cv::Mat3b &, ITMUChar4Image *): (h, w, 3) BGR8 into (h, w, 4) RGBA8 with alpha 255."""
+        ViewBuilder._inputs_ready()
+        h, w = bgr.shape[:2]
+        self.e.check(self.e.lib.b200_bgr_to_rgba(self.e.h, _ptr(out_rgba), _ptr(bgr), w, h))
 
 
 class ViewBuilder:

@@ -17,6 +17,7 @@ KITTI_W, KITTI_H = 1242, 375
 KITTI_FX = KITTI_FY = 707.0912
 KITTI_CX = 601.8873 * 1242.0 / 1226.0
 KITTI_CY = 183.1104 * 375.0 / 370.0
+KITTI_BASELINE_M = 0.5372   # the KITTI stereo rig's colour-camera baseline (DS/Input.h's StereoCalibration for the odometry sequences)
 
 
 def _rot_y(a):
@@ -124,6 +125,16 @@ def kitti_frame(scene, frame, w=KITTI_W, h=KITTI_H, zmax=20.0, scale=1.0, **kw):
     M = kitti_pose(frame)
     out = scene.render(M, ww, hh, float(proj[0]), float(proj[1]), float(proj[2]), float(proj[3]), zmax=zmax, **kw)
     return out + (M, proj)
+
+
+def stereo_frame(depth, rgb, focal_length_px=KITTI_FX, baseline_m=KITTI_BASELINE_M):
+    """DynSLAM's stored stereo input for a rendered frame: OpenCV's BGR8 image (h, w, 3) of `rgb` and the float32 disparity
+    f * b / depth a DispNet PFM holds (0 where there is no depth)."""
+    bgr = np.ascontiguousarray(rgb[..., 2::-1])
+    fb = np.float32(focal_length_px) * np.float32(baseline_m)
+    with np.errstate(divide="ignore"):
+        disp = np.where(depth > 0, fb / np.maximum(depth, np.float32(1e-30)), np.float32(0.0)).astype(np.float32)
+    return bgr, disp
 
 
 def plane_frame(seed=1, w=640, h=480, z0=1.5, ripple=0.1, holes=0.02):

@@ -306,6 +306,40 @@ b200_status b200_host_frame_submit_raw(b200_engine *e, b200_scene *scene, b200_r
                                        b200_vec4f *d_points, b200_vec4f *d_normals, const b200_frame_opts *opts,
                                        b200_vec4u *h_outImage, int slot);
 
+/* ---- DynSLAM's stored stereo input (DS/Input.cpp:41-97 -> DS/InfiniTamDriver.cpp:81-100) -------------------------------
+   The two host loops every DynSLAM frame passes through before InfiniTamDriver::UpdateView, on the device and bit-exact:
+   the int16 millimetre depth image from the stored DispNet disparity (DepthProvider::DepthFromDisparityMap<float> with
+   scale 1, DS/DepthProvider.h:94-137, around PrecomputedDepthProvider::DepthFromDisparity, DS/PrecomputedDepthProvider.cpp:
+   77-80) or from the stored ELAS depth (the max-depth clamp of PrecomputedDepthProvider::ReadPrecomputed, :52-74), and the
+   RGBA8 colour image from OpenCV's BGR8 frame (CvToItm(const cv::Mat3b &, ...), DS/InfiniTamDriver.cpp:81-100). */
+
+enum { B200_DEPTH_IN_DISPARITY_F32 = 0, B200_DEPTH_IN_DEPTH_MM_S16 = 1 };
+
+typedef struct {
+  int32_t kind;                /* B200_DEPTH_IN_*: 0 float32 disparity in px (DispNet PFM), 1 int16 depth in mm (ELAS XML) */
+  float baseline_m;            /* dynslam::StereoCalibration::baseline_meters (DS/DepthProvider.h:22-28; kind 0 only) */
+  float focal_length_px;       /* dynslam::StereoCalibration::focal_length_px (kind 0 only) */
+  float min_depth_m;           /* DepthProvider::min_depth_m_ (kind 0 only: the clamp of kind 1 has no lower bound) */
+  float max_depth_m;           /* DepthProvider::max_depth_m_; (int32)(max_depth_m * 1000) must be below 32767 */
+} b200_depth_input;
+
+/* d_out_mm (w*h int16) from d_in (w*h float disparities or int16 millimetres, per kind). A depth of (int32)(1000 * focal *
+   baseline / disp) outside [(int32)(min_depth_m * 1000), (int32)(max_depth_m * 1000)] becomes 0, as does every |disp| < 1
+   (the reference's unqualified abs() is int abs(int)); kind 1 sets values above (int16)round(max_depth_m * 1000) to 0.
+   d_out_mm may equal d_in for kind 1. Synchronous. */
+b200_status b200_depth_mm_from_input(b200_engine *e, int16_t *d_out_mm, const void *d_in, int w, int h, const b200_depth_input *in);
+/* CvToItm(const cv::Mat3b &, ITMUChar4Image *): d_bgr (w*h*3 bytes) into d_out (w*h RGBA8, a = 255). Synchronous. */
+b200_status b200_bgr_to_rgba(b200_engine *e, b200_vec4u *d_out, const uint8_t *d_bgr, int w, int h);
+/* b200_host_frame_submit_raw from the stored stereo input: h_depthIn (view->depth_w x depth_h, float disparity or int16 mm
+   per in->kind) and h_bgr (view->rgb_w x rgb_h BGR8) are copied H2D; on the copy stream one kernel turns them into the int16
+   mm depth and the RGBA8 colour image; then UpdateView and the fused frame run as in b200_host_frame_submit_raw. If
+   d_depthMmOut is not NULL it receives the frame's int16 mm depth (the input depth of b200_evaluate_depth); it is complete
+   when b200_host_frame_wait(slot) returns. Same slot rules as b200_host_frame_submit; modelSensorNoise is rejected. */
+b200_status b200_host_frame_submit_stereo(b200_engine *e, b200_scene *scene, b200_render_state *rs, b200_view *view,
+                                          const uint8_t *h_bgr, const void *h_depthIn, const b200_depth_input *in,
+                                          const b200_view_calib *calib, b200_vec4f *d_points, b200_vec4f *d_normals,
+                                          const b200_frame_opts *opts, b200_vec4u *h_outImage, int16_t *d_depthMmOut, int slot);
+
 /* ---- instance frame splitting (SURVEY 8(f) rank 2) ---------------------------------------------------
    Replaces the download / CPU masking / upload round trip of InstanceReconstructor::ProcessFrame
    (DS/InstRecLib/InstanceReconstructor.cpp:180-197) around ProcessSilhouette_CPU / RemoveSilhouette_CPU
