@@ -33,6 +33,23 @@ VOXEL_DTYPE = np.dtype([("sdf", np.int16), ("w_depth", np.uint8), ("clr", np.uin
                         ("w_color", np.uint8), ("_pad", np.uint8)])
 assert HASH_ENTRY_DTYPE.itemsize == 20 and VOXEL_DTYPE.itemsize == 8
 
+# b200_checkpoint_header and its section order (include/b200fusion.h)
+CHECKPOINT_MAGIC, CHECKPOINT_VERSION, CHECKPOINT_HEADER_BYTES = b"B200CKPT", 1, 512
+CHECKPOINT_SECTIONS = ["HASH_INDEX", "HASH_ENTRIES", "ALLOCATION_LIST", "EXCESS_LIST", "SWAP_STATES", "VIS_INDEX", "VIS_VALUE",
+                       "VISIBLE_LIST", "MINMAX", "RAYCAST_RESULT", "RAYCAST_IMAGE", "FWD_PROJECTION", "FWD_MISSING", "QUEUE_COUNTS",
+                       "QUEUE_ITEMS", "BLOCK_IDS", "BLOCK_DATA"]
+CK_HAS_SWAP_STATES, CK_HAS_FORWARD = 1, 2
+CHECKPOINT_HEADER_DTYPE = np.dtype([
+    ("magic", "S8"), ("version", "<u4"), ("flags", "<u4"),
+    ("numBlocks", "<i4"), ("numBuckets", "<i4"), ("excessSize", "<i4"), ("img_w", "<i4"), ("img_h", "<i4"),
+    ("voxelSize", "<f4"), ("mu", "<f4"), ("maxW", "<i4"), ("viewFrustum_min", "<f4"), ("viewFrustum_max", "<f4"),
+    ("stopIntegratingAtMaxW", "<i4"), ("useSwapping", "<i4"),
+    ("lastFreeBlockId", "<i4"), ("lastFreeExcessListId", "<i4"), ("noVisibleBlocks", "<i4"), ("noFwdProjMissingPoints", "<i4"),
+    ("frameIdx", "<i4"), ("noSnapshots", "<i4"), ("totalDecayed", "<i8"), ("droppedSnapshots", "<i8"),
+    ("noEntries", "<i8"), ("noVisBytes", "<i8"), ("noBlocks", "<i8"), ("noQueueItems", "<i8"), ("totalBytes", "<u8"),
+    ("section", "<u8", (len(CHECKPOINT_SECTIONS), 2)), ("reserved", "u1", 96)])
+assert CHECKPOINT_HEADER_DTYPE.itemsize == CHECKPOINT_HEADER_BYTES
+
 f16 = C.c_float * 16
 f4 = C.c_float * 4
 
@@ -164,7 +181,7 @@ EXPORTS = [
     "b200_depth_mm_from_input", "b200_bgr_to_rgba", "b200_host_frame_submit_stereo",
     "b200_process_silhouettes", "b200_process_silhouettes_async", "b200_composite_depth", "b200_composite_color",
     "b200_composite_instances", "b200_evaluate_depth",
-    "b200_mesh_scene", "b200_comm_unique_id", "b200_comm_create", "b200_comm_destroy", "b200_comm_last_error", "b200_gather_composite_submit",
+    "b200_mesh_scene", "b200_checkpoint_save", "b200_checkpoint_load", "b200_comm_unique_id", "b200_comm_create", "b200_comm_destroy", "b200_comm_last_error", "b200_gather_composite_submit",
     "b200_gather_composite_release", "b200_gather_composite_wait",
 ]
 # measurement / test hooks (include/b200fusion_diag.h): exported by the same library, not part of the drop-in boundary
@@ -235,6 +252,8 @@ def load_library():
     lib.b200_composite_color.argtypes = [vp, vp, vp, vp, vp, C.c_int, P(C.c_int32), C.c_float]
     lib.b200_composite_instances.argtypes = [vp, vp, vp, C.c_int, P(InstanceLayer), C.c_int, C.c_float, C.c_float]
     lib.b200_mesh_scene.argtypes = [vp, P(Scene), vp, C.c_uint32, P(C.c_uint32)]
+    lib.b200_checkpoint_save.argtypes = [vp, P(Scene), P(RenderState), vp, C.c_size_t, P(C.c_size_t)]
+    lib.b200_checkpoint_load.argtypes = [vp, P(Scene), P(RenderState), vp, C.c_size_t]
     lib.b200_evaluate_depth.argtypes = [vp, P(EvalParams), vp, C.c_int, vp, vp, vp, P(EvalCallback), C.c_int, P(EvalResult), P(EvalResult), P(EvalSummary)]
     lib.b200_comm_unique_id.argtypes = [C.c_char_p]
     lib.b200_comm_create.argtypes = [C.c_int, C.c_int, C.c_int, C.c_char_p, C.c_int, C.c_int, P(vp)]

@@ -340,11 +340,16 @@ __global__ void k_find_allocated(const b200_hash_entry *__restrict__ table, int 
   }
 }
 
-// b200_diag_push_decay_snapshot: n caller positions appended to the ring as snapshot `slot` (one CTA: the cursor is read
-// before and moved after every item is written)
+// b200_diag_push_decay_snapshot / b200_checkpoint_load: n caller positions appended to the ring as snapshot `slot` (one CTA:
+// the cursor is read before and moved after every item is written). n == -1: a snapshot that is already overwritten — it
+// starts more than ringCap items behind the cursor and takes no room, so k_decay_blocks sweeps nothing for it.
 __global__ void k_push_snapshot(const b200_vec3i *positions, int n, b200_vec3i *ring, long long ringCap, long long *snapStart,
                                 int *snapCount, int slot, DevCounters *ctr) {
   const long long ringStart = ctr->ringHead;
+  if (n < 0) {
+    if (threadIdx.x == 0) { snapStart[slot] = ringStart - ringCap - 1; snapCount[slot] = 0; }
+    return;
+  }
   for (int i = threadIdx.x; i < n; i += blockDim.x) ring[(ringStart + i) % ringCap] = positions[i];
   __syncthreads();
   if (threadIdx.x == 0) publish_snapshot(ctr, snapStart, snapCount, slot, ringStart, n);

@@ -40,7 +40,7 @@ static void mat_mul(const float *lhs, const float *rhs, float *out) {
   memcpy(out, r, sizeof(r));
 }
 
-static SceneRef scene_ref(const b200_scene *s, const b200_render_state *rs) {
+SceneRef scene_ref(const b200_scene *s, const b200_render_state *rs) {
   SceneRef r;
   r.voxels = s->d_voxels; r.allocationList = s->d_allocationList; r.hash = s->d_hash; r.excessList = s->d_excessList;
   r.swapStates = s->d_swapStates;
@@ -63,7 +63,7 @@ static FrameGeom frame_geom(const b200_scene *s, const b200_view *v) {
   return g;
 }
 
-static b200_status check_scene(b200_engine *e, const b200_scene *s) {
+b200_status check_scene(b200_engine *e, const b200_scene *s) {
   if (!s || s->numBlocks > e->numBlocks || s->numBuckets != e->numBuckets || s->excessSize != e->excessSize ||
       (s->numBuckets & (s->numBuckets - 1))) {
     snprintf(e->err, sizeof(e->err), "scene sizes do not match the engine configuration");
@@ -83,7 +83,7 @@ static b200_status upload(b200_engine *e, const b200_scene *s, const b200_render
   return B200_OK;
 }
 
-static b200_status download_sync(b200_engine *e, b200_scene *s, b200_render_state *rs) {
+b200_status download_sync(b200_engine *e, b200_scene *s, b200_render_state *rs) {
   CK(cudaMemcpyAsync(e->h_ctr, e->d_ctr, sizeof(DevCounters), cudaMemcpyDeviceToHost, e->stream));
   CK(cudaStreamSynchronize(e->stream));
   CK(cudaGetLastError());
@@ -228,6 +228,7 @@ void b200_engine_destroy(b200_engine *e) {
   if (e->evRing) { for (int i = 0; i < e->evRingCap * 2; ++i) cudaEventDestroy(e->evRing[i]); free(e->evRing); }
   if (e->traceEv) { for (int i = 0; i < e->traceCap * 2; ++i) cudaEventDestroy(e->traceEv[i]); free(e->traceEv); free(e->traceName); }
   cudaGetLastError();
+  checkpoint_release(e);
   if (e->ownStream && e->stream) cudaStreamDestroy(e->stream);
   delete e;
 }
@@ -306,7 +307,7 @@ b200_status b200_reset_scene(b200_engine *e, b200_scene *s) {
 // When Decay() is never called (--voxel_decay=false) or min_decay_age is very large, the OLDEST snapshot is dropped to make
 // room — never an error (the ring's item overflow is handled the same way on the device: decay.cu recognises an overwritten
 // snapshot by its start position and sweeps nothing).
-static int push_snapshot_slot(b200_engine *e) {
+int push_snapshot_slot(b200_engine *e) {
   if (e->qSize >= SNAP_SLOTS - 1) { e->qHead++; e->qSize--; e->droppedSnapshots++; }
   const int slot = (e->qHead + e->qSize) % SNAP_SLOTS;
   e->qSize++;

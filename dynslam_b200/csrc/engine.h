@@ -105,19 +105,28 @@ struct b200_engine {
   int rcTileLog2, rcOrder, rcImpl;    // B200_RC_TILE=0..5 (3: 8x4), B200_RC_ORDER=0|1 (1), B200_RC_IMPL=old (1: neighbourhood cache)
   int lastIntegrateKernel, lastIntegrateGrid;   // what the last launch_integrate ran (b200_diag_last_integrate)
   bool hostAuthoritative;            // host copies of the counters are newer than the device ones
+  struct CheckpointScratch *ck;      // checkpoint.cu: staging, bounce buffers and the kept classification (allocated on first use)
   char err[512];
 };
+
+// engine.cu helpers shared with checkpoint.cu
+SceneRef scene_ref(const b200_scene *s, const b200_render_state *rs);
+b200_status check_scene(b200_engine *e, const b200_scene *s);
+b200_status download_sync(b200_engine *e, b200_scene *s, b200_render_state *rs);
+extern "C" int push_snapshot_slot(b200_engine *e);   // (defined inside engine.cu's extern "C" block)
+void checkpoint_release(b200_engine *e);
 
 #define SNAP_SLOTS 4096
 
 // Device half of a decay-queue push (Reco_CUDA.cu:302-316): the `kept` positions written to the ring from ringStart on
-// become snapshot `slot`, and the ring's cursor moves past them. Allocation's list pass and b200_diag_push_decay_snapshot
-// both publish through here; the host half is push_snapshot_slot (engine.cu).
+// become snapshot `slot`, and the ring's cursor moves past them. Allocation's list pass, b200_diag_push_decay_snapshot and
+// b200_checkpoint_load all publish through here; the host half is push_snapshot_slot (engine.cu).
 DEV void publish_snapshot(DevCounters *ctr, long long *snapStart, int *snapCount, int slot, long long ringStart, int kept) {
   snapStart[slot] = ringStart;
   snapCount[slot] = kept;
   ctr->ringHead = ringStart + kept;
 }
+// n == -1 pushes a snapshot the ring has already overwritten: its Decay sweeps nothing and counts it as dropped
 void launch_push_snapshot(b200_engine *e, const b200_vec3i *positions, int n, int snapSlot);
 
 // launchers (each enqueues on e->stream and bumps e->launches)

@@ -236,6 +236,25 @@ class Engine:
         self.check(self.lib.b200_diag_push_decay_snapshot(self.h, _ptr(positions) if positions.numel() else None,
                                                           positions.shape[0]))
 
+    def save_checkpoint(self, scene, renderState):
+        """b200_checkpoint_save: the volume's state (scene, render state, frame index, decay queue) as a uint8 array, laid out as
+        include/b200fusion.h documents; load_checkpoint resumes fusion from it bit for bit. Finishes outstanding frames first."""
+        n = C.c_size_t()
+        self.after_torch()
+        self.check(self.lib.b200_checkpoint_save(self.h, C.byref(scene.c), C.byref(renderState.c), None, 0, C.byref(n)))
+        buf = np.empty(n.value, dtype=np.uint8)
+        self.check(self.lib.b200_checkpoint_save(self.h, C.byref(scene.c), C.byref(renderState.c), buf.ctypes.data, buf.size,
+                                                 C.byref(n)))
+        return buf
+
+    def load_checkpoint(self, scene, renderState, buf):
+        """b200_checkpoint_load: replaces the state of scene and renderState (same geometry, voxelSize, mu and optional buffers)
+        and this engine's frame index and decay queue with a checkpoint's. Raises ValueError, with nothing written, on a buffer
+        that does not fit."""
+        b = np.ascontiguousarray(np.frombuffer(memoryview(buf).cast("B"), dtype=np.uint8))
+        self.after_torch()
+        self.check(self.lib.b200_checkpoint_load(self.h, C.byref(scene.c), C.byref(renderState.c), b.ctypes.data, b.size))
+
     def set_frame_index(self, f):
         """test hook (include/b200fusion_diag.h): the frame index Decay measures block ages against"""
         self.lib.b200_diag_set_frame_index(self.h, int(f))

@@ -57,6 +57,20 @@ def read_mask_txt(path, width, height):
     return out
 
 
+def checkpoint_header(buf):
+    """The b200_checkpoint_header of a checkpoint (Engine.save_checkpoint, b200_checkpoint_save) as a dict, with "sections" mapping
+    each section name to (offset, length) in bytes. Reads only the header; b200_checkpoint_load checks the rest."""
+    b = np.frombuffer(memoryview(buf).cast("B"), dtype=np.uint8)
+    if b.size < abi.CHECKPOINT_HEADER_BYTES:
+        raise ValueError(f"{b.size} bytes: shorter than the {abi.CHECKPOINT_HEADER_BYTES}-byte checkpoint header")
+    h = b[:abi.CHECKPOINT_HEADER_BYTES].view(abi.CHECKPOINT_HEADER_DTYPE)[0]
+    if bytes(h["magic"]) != abi.CHECKPOINT_MAGIC:
+        raise ValueError("not a checkpoint (bad magic)")
+    out = {k: h[k].item() for k in abi.CHECKPOINT_HEADER_DTYPE.names if k not in ("magic", "section", "reserved")}
+    out["sections"] = {n: (int(h["section"][i, 0]), int(h["section"][i, 1])) for i, n in enumerate(abi.CHECKPOINT_SECTIONS)}
+    return out
+
+
 def write_obj(path, triangles, noTotalTriangles=None, noMaxTriangles=None):
     """ITMMesh::WriteOBJ (ITMLib/Objects/ITMMesh.h:46-122) on an array of abi.TRIANGLE_DTYPE."""
     h = abi.host_library()

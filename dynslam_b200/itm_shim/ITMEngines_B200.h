@@ -212,6 +212,44 @@ class ITMSceneReconstructionEngine_B200<TVoxel, ITMVoxelBlockHash> : public ITMS
   }
 
   size_t GetDecayedBlockCount() override { return b200_decayed_block_count(h->e); }
+
+  /// Writes the volume's checkpoint (include/b200fusion.h: scene, render state, frame index, decay queue) to `path`, the
+  /// buffer verbatim. Returns false if the file cannot be written.
+  bool SaveScene(ITMScene<TVoxel, ITMVoxelBlockHash> *scene, ITMRenderState *renderState, const char *path) {
+    b200_scene s = b200_detail::PackScene(scene);
+    b200_render_state r = b200_detail::PackRenderState(renderState);
+    size_t size = 0;
+    h->check(b200_checkpoint_save(h->e, &s, &r, nullptr, 0, &size));
+    std::unique_ptr<char[]> buf(new char[size]);
+    h->check(b200_checkpoint_save(h->e, &s, &r, buf.get(), size, &size));
+    FILE *f = fopen(path, "wb");
+    if (!f) return false;
+    const bool ok = fwrite(buf.get(), 1, size, f) == size;
+    return (fclose(f) == 0) && ok;
+  }
+
+  /// Replaces the volume's state with the checkpoint in `path` (same scene geometry, voxelSize and mu); fusion then continues
+  /// bit for bit as in the process that saved it. Returns false, with the volume untouched, if the file cannot be read or is
+  /// not a checkpoint that fits this scene (the reason is printed and stays in b200_last_error); CUDA errors exit as elsewhere.
+  bool LoadScene(ITMScene<TVoxel, ITMVoxelBlockHash> *scene, ITMRenderState *renderState, const char *path) {
+    FILE *f = fopen(path, "rb");
+    if (!f) return false;
+    fseek(f, 0, SEEK_END);
+    const long size = ftell(f);
+    fseek(f, 0, SEEK_SET);
+    std::unique_ptr<char[]> buf(new char[size > 0 ? size : 1]);
+    const bool ok = size > 0 && fread(buf.get(), 1, (size_t)size, f) == (size_t)size;
+    fclose(f);
+    if (!ok) return false;
+    b200_scene s = b200_detail::PackScene(scene);
+    b200_render_state r = b200_detail::PackRenderState(renderState);
+    const b200_status st = b200_checkpoint_load(h->e, &s, &r, buf.get(), (size_t)size);
+    if (st == B200_ERR_INVALID) { fprintf(stderr, "b200fusion: %s: %s\n", path, b200_last_error(h->e)); return false; }
+    h->check(st);
+    b200_detail::UnpackScene(s, scene);
+    b200_detail::UnpackRenderState(r, renderState);
+    return true;
+  }
 };
 
 // --------------------------------------------------------------------------------------------------

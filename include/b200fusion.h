@@ -437,6 +437,81 @@ typedef struct { float p0[3], p1[3], p2[3], c0[3], c1[3], c2[3]; } b200_triangle
 b200_status b200_mesh_scene(b200_engine *e, const b200_scene *scene, b200_triangle *d_triangles, uint32_t noMaxTriangles,
                             uint32_t *noTotalTriangles);
 
+/* ---- checkpoints: one volume's state saved to a host buffer and loaded back (no reference twin) ------------------------
+   A checkpoint holds everything that decides the future of one volume and nothing that can be derived: after a load, fusion
+   continues bit for bit as if the process had never stopped. It holds no device pointers or ordinals, so it can be loaded on
+   another GPU or in another process; the same state always gives the same bytes (save -> load -> save is identical).
+
+   Layout (little-endian). A 512-byte b200_checkpoint_header, then the sections below in this order, each 16-byte aligned, the
+   voxel payload 4096-byte aligned; the header's section table gives every offset and length, padding bytes are zero:
+     HASH_INDEX      uint32 x noEntries       ascending indices of the hash entries that differ from the reset entry
+                                              {pos 0, pad 0, offset 0, ptr -2, allocatedTime 0} (stale pos/offset of freed heads count)
+     HASH_ENTRIES    20 B x noEntries         those entries (b200_hash_entry)
+     ALLOCATION_LIST int32 x numBlocks        localVBA's free list, in full
+     EXCESS_LIST     int32 x excessSize       the excess list, in full
+     SWAP_STATES     uint8 x (numBuckets + excessSize), only with B200_CK_HAS_SWAP_STATES
+     VIS_INDEX       uint32 x noVisBytes      ascending indices of the nonzero entriesVisibleType bytes
+     VIS_VALUE       uint8 x noVisBytes       their values
+     VISIBLE_LIST    12 B x min(noVisibleBlocks, numBlocks)
+     MINMAX          8 B x img_w*img_h        renderingRangeImage
+     RAYCAST_RESULT  16 B x img_w*img_h
+     RAYCAST_IMAGE   4 B x img_w*img_h
+     FWD_PROJECTION  16 B x img_w*img_h, FWD_MISSING int32 x img_w*img_h: only with B200_CK_HAS_FORWARD
+     QUEUE_COUNTS    int32 x noSnapshots      the decay queue, oldest first: items per snapshot, -1 = overwritten in the ring
+                                              before the save (b200_engine_config.decayRingItems; its Decay sweeps nothing)
+     QUEUE_ITEMS     12 B x noQueueItems      the snapshots' block positions, oldest first
+     BLOCK_IDS       uint32 x noBlocks        ascending ids of the voxel blocks that differ from a reset block {sdf 32767, 0...},
+                                              allocated or not (decay can free a block whose voxels still hold sdf and colour)
+     BLOCK_DATA      4096 B x noBlocks        those blocks
+   Not saved: the engine's cache of the visible list's VBA pointers (the next integration looks the blocks up itself). */
+
+#define B200_CHECKPOINT_MAGIC "B200CKPT"
+#define B200_CHECKPOINT_VERSION 1
+#define B200_CHECKPOINT_HEADER_BYTES 512
+enum {
+  B200_CK_HASH_INDEX, B200_CK_HASH_ENTRIES, B200_CK_ALLOCATION_LIST, B200_CK_EXCESS_LIST, B200_CK_SWAP_STATES, B200_CK_VIS_INDEX,
+  B200_CK_VIS_VALUE, B200_CK_VISIBLE_LIST, B200_CK_MINMAX, B200_CK_RAYCAST_RESULT, B200_CK_RAYCAST_IMAGE, B200_CK_FWD_PROJECTION,
+  B200_CK_FWD_MISSING, B200_CK_QUEUE_COUNTS, B200_CK_QUEUE_ITEMS, B200_CK_BLOCK_IDS, B200_CK_BLOCK_DATA, B200_CK_SECTIONS
+};
+#define B200_CK_HAS_SWAP_STATES 1u
+#define B200_CK_HAS_FORWARD 2u
+
+typedef struct {
+  char magic[8];                       /* B200_CHECKPOINT_MAGIC, no terminator */
+  uint32_t version, flags;             /* B200_CHECKPOINT_VERSION; B200_CK_HAS_* */
+  int32_t numBlocks, numBuckets, excessSize, img_w, img_h;   /* geometry: must equal the loading scene's and render state's */
+  float voxelSize, mu;                 /* must equal the loading scene's, bit for bit */
+  int32_t maxW; float viewFrustum_min, viewFrustum_max; int32_t stopIntegratingAtMaxW, useSwapping;   /* for information only */
+  int32_t lastFreeBlockId, lastFreeExcessListId, noVisibleBlocks, noFwdProjMissingPoints;
+  int32_t frameIdx, noSnapshots;
+  int64_t totalDecayed, droppedSnapshots;
+  int64_t noEntries, noVisBytes, noBlocks, noQueueItems;
+  uint64_t totalBytes;
+  uint64_t section[B200_CK_SECTIONS][2];   /* offset, length in bytes */
+  uint8_t reserved[96];
+} b200_checkpoint_header;
+
+/* Save. First brings the engine to the b200_sync() state (outstanding frames finished, the expected-depth image complete).
+   h_out == NULL: only *size is set. Every such size query classifies the state afresh, and the save with h_out that
+   immediately follows it reuses that classification instead of sweeping the voxel block array again (any engine call that
+   launches work in between discards it; a save with h_out != NULL and no size query before it classifies on its own). After
+   a change the caller makes to the buffers itself, which the engine cannot see, a size query therefore brings the saved
+   state up to date. h_out may be pageable or pinned; capacity below *size is B200_ERR_INVALID and nothing is written.
+   Synchronous. */
+b200_status b200_checkpoint_save(b200_engine *e, b200_scene *scene, b200_render_state *rs, void *h_out, size_t capacity,
+                                 size_t *size);
+/* Load into a scene and render state of the same geometry, voxelSize and mu, with the same optional buffers (swap states,
+   forward projection). Writes every saved buffer (the rest of the voxel blocks, hash entries and visibility bytes get their
+   reset values), the host counters of scene and rs, and the engine's frame index, decay counters and queue. A queue longer
+   than this engine's ring or 4095-frame queue holds drops its oldest snapshots, as a running engine does. Every rejection
+   (B200_ERR_INVALID: bad magic or version, a truncated buffer or section table, a geometry, voxelSize, mu or optional-buffer
+   mismatch, an index or count out of range or out of order, a host-frame slot not yet waited for) is made before anything
+   is written. A checkpoint is trusted data beyond that: the values inside its sections (hash entries, free-list entries,
+   voxels, images) are loaded as they are, without range checks or a checksum. Clears the engine's allocation request keys,
+   which are tagged with frame indices, so a checkpoint of an earlier frame loads into an engine that has run past it.
+   Synchronous. */
+b200_status b200_checkpoint_load(b200_engine *e, b200_scene *scene, b200_render_state *rs, const void *h_in, size_t size);
+
 /* ---- the exchange step of the multi-volume configuration (SURVEY 8e) -----------------------------------------------
    One volume per GPU, one process per GPU: the static map on rank 0, one ITMScene per car on the other ranks
    (DS/InstRecLib/InstanceReconstructor.cpp:363-389). Fusion, allocation and decay need no communication; per frame every
