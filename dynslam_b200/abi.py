@@ -183,6 +183,7 @@ EXPORTS = [
     "b200_composite_instances", "b200_evaluate_depth",
     "b200_mesh_scene", "b200_checkpoint_save", "b200_checkpoint_load", "b200_comm_unique_id", "b200_comm_create", "b200_comm_destroy", "b200_comm_last_error", "b200_gather_composite_submit",
     "b200_gather_composite_release", "b200_gather_composite_wait",
+    "b200_render_view_async", "b200_render_view_sync", "b200_render_view_submit", "b200_render_view_wait", "b200_engine_wait_engine",
 ]
 # measurement / test hooks (include/b200fusion_diag.h): exported by the same library, not part of the drop-in boundary
 DIAG_EXPORTS = ["b200_set_timing", "b200_get_trace", "b200_get_stats", "b200_selftest_divide", "b200_diag_set_max_rendering_blocks",
@@ -264,6 +265,11 @@ def load_library():
     lib.b200_gather_composite_submit.argtypes = [vp, vp, vp, vp, vp, vp, P(C.c_int32), C.c_float, C.c_float, C.c_int]
     lib.b200_gather_composite_release.argtypes = [vp, vp, C.c_int]
     lib.b200_gather_composite_wait.argtypes = [vp, C.c_int]
+    lib.b200_render_view_async.argtypes = [vp, P(Scene), P(RenderState), P(Camera), C.c_int, vp, vp]
+    lib.b200_render_view_sync.argtypes = [vp, P(RenderState)]
+    lib.b200_render_view_submit.argtypes = [vp, P(Scene), P(RenderState), P(Camera), C.c_int, vp, vp, C.c_int]
+    lib.b200_render_view_wait.argtypes = [vp, C.c_int]
+    lib.b200_engine_wait_engine.argtypes = [vp, vp]
     lib.b200_set_timing.argtypes = [vp, C.c_int]
     lib.b200_set_timing.restype = None
     lib.b200_get_stats.argtypes = [vp, P(FrameStats)]

@@ -44,32 +44,6 @@ void launch_reset(b200_engine *e, const SceneRef &s) {
   e->launches++;
 }
 
-// ------------------------------------------------------------------------------------------------
-// visibility test (DA/ITMSceneReconstructionEngine.h:315-397)
-// ------------------------------------------------------------------------------------------------
-DEV bool point_visible(const Mat4 &M, const float *proj, float x, float y, float z, int w, int h) {
-  Vec4 b = m4v4(M, x, y, z, 1.0f);
-  if (b.z < 1e-10f) return false;
-  float u = proj[0] * b.x / b.z + proj[2];
-  float v = proj[1] * b.y / b.z + proj[3];
-  return (u >= 0 && u < w && v >= 0 && v < h);
-}
-
-// checkBlockVisibility<false>: corner order and the incremental +=/-= updates are part of the arithmetic contract
-__device__ bool block_visible(int bx, int by, int bz, const Mat4 &M, const float *proj, float voxelSize, int w, int h) {
-  const float factor = (float)BS * voxelSize;
-  float x = (float)bx * factor, y = (float)by * factor, z = (float)bz * factor;
-  if (point_visible(M, proj, x, y, z, w, h)) return true;
-  z += factor; if (point_visible(M, proj, x, y, z, w, h)) return true;
-  y += factor; if (point_visible(M, proj, x, y, z, w, h)) return true;
-  x += factor; if (point_visible(M, proj, x, y, z, w, h)) return true;
-  z -= factor; if (point_visible(M, proj, x, y, z, w, h)) return true;
-  y -= factor; if (point_visible(M, proj, x, y, z, w, h)) return true;
-  x -= factor; y += factor; if (point_visible(M, proj, x, y, z, w, h)) return true;
-  x += factor; y -= factor; z += factor; if (point_visible(M, proj, x, y, z, w, h)) return true;
-  return false;
-}
-
 // Transient visibility codes, only alive between the two kernels of ONE allocate call: the reference marks every
 // previously visible block 3 (setToType3) and re-tests the survivors' frustum visibility inside the full-table sweep.
 // Here the re-test is done eagerly, one previously visible block per thread, and its verdict is parked in the byte; the

@@ -214,6 +214,32 @@ DEV void atomic_min_posf(float *a, float v) { atomicMin(reinterpret_cast<int *>(
 DEV void atomic_max_posf(float *a, float v) { atomicMax(reinterpret_cast<int *>(a), __float_as_int(v)); }
 
 // ------------------------------------------------------------------------------------------------
+// visibility test (DA/ITMSceneReconstructionEngine.h:315-397): alloc.cu's sweeps and the free-view preview (preview.cu)
+// ------------------------------------------------------------------------------------------------
+DEV bool point_visible(const Mat4 &M, const float *proj, float x, float y, float z, int w, int h) {
+  Vec4 b = m4v4(M, x, y, z, 1.0f);
+  if (b.z < 1e-10f) return false;
+  float u = proj[0] * b.x / b.z + proj[2];
+  float v = proj[1] * b.y / b.z + proj[3];
+  return (u >= 0 && u < w && v >= 0 && v < h);
+}
+
+// checkBlockVisibility<false>: corner order and the incremental +=/-= updates are part of the arithmetic contract
+__device__ inline bool block_visible(int bx, int by, int bz, const Mat4 &M, const float *proj, float voxelSize, int w, int h) {
+  const float factor = (float)BS * voxelSize;
+  float x = (float)bx * factor, y = (float)by * factor, z = (float)bz * factor;
+  if (point_visible(M, proj, x, y, z, w, h)) return true;
+  z += factor; if (point_visible(M, proj, x, y, z, w, h)) return true;
+  y += factor; if (point_visible(M, proj, x, y, z, w, h)) return true;
+  x += factor; if (point_visible(M, proj, x, y, z, w, h)) return true;
+  z -= factor; if (point_visible(M, proj, x, y, z, w, h)) return true;
+  y -= factor; if (point_visible(M, proj, x, y, z, w, h)) return true;
+  x -= factor; y += factor; if (point_visible(M, proj, x, y, z, w, h)) return true;
+  x += factor; y -= factor; z += factor; if (point_visible(M, proj, x, y, z, w, h)) return true;
+  return false;
+}
+
+// ------------------------------------------------------------------------------------------------
 // expected depths: block projection shared by vis.cu (k_project_blocks) and alloc.cu (k_visible_list)
 // ------------------------------------------------------------------------------------------------
 // ProjectSingleBlock — DA/ITMVisualisationEngine.h:29-71

@@ -229,6 +229,7 @@ void b200_engine_destroy(b200_engine *e) {
   if (e->traceEv) { for (int i = 0; i < e->traceCap * 2; ++i) cudaEventDestroy(e->traceEv[i]); free(e->traceEv); free(e->traceName); }
   cudaGetLastError();
   checkpoint_release(e);
+  preview_release(e);
   if (e->ownStream && e->stream) cudaStreamDestroy(e->stream);
   delete e;
 }

@@ -106,6 +106,7 @@ struct b200_engine {
   int lastIntegrateKernel, lastIntegrateGrid;   // what the last launch_integrate ran (b200_diag_last_integrate)
   bool hostAuthoritative;            // host copies of the counters are newer than the device ones
   struct CheckpointScratch *ck;      // checkpoint.cu: staging, bounce buffers and the kept classification (allocated on first use)
+  struct PreviewScratch *pv;         // preview.cu: the free-view preview's own counters, scan descriptors and hand-over slots (allocated on first use)
   char err[512];
 };
 
@@ -115,6 +116,7 @@ b200_status check_scene(b200_engine *e, const b200_scene *s);
 b200_status download_sync(b200_engine *e, b200_scene *s, b200_render_state *rs);
 extern "C" int push_snapshot_slot(b200_engine *e);   // (defined inside engine.cu's extern "C" block)
 void checkpoint_release(b200_engine *e);
+void preview_release(b200_engine *e);
 
 #define SNAP_SLOTS 4096
 

@@ -336,6 +336,11 @@ class Engine:
     def host_frame_wait(self, slot):
         self.check(self.lib.b200_host_frame_wait(self.h, slot))
 
+    def wait_engine(self, other):
+        """b200_engine_wait_engine: this engine's stream waits, on the device, for what is enqueued on other's stream so far
+        (compositing layers another engine rendered without a host synchronisation in between)."""
+        self.check(self.lib.b200_engine_wait_engine(self.h, other.h))
+
 
 def make_view_calib(trafoType=1, params=(1.0 / 1000.0, 0.0), fx_depth=0.0, intrinsics_d=(0.0, 0.0, 0.0, 0.0), useBilateralFilter=True,
                     modelSensorNoise=False):
@@ -548,6 +553,29 @@ class VisualisationEngine:
         self.e.after_torch()
         self.e.check(self.e.lib.b200_render_image(self.e.h, C.byref(self.scene.c), C.byref(renderState.c), C.byref(camera),
                                                    _ptr(outputCharImage), _ptr(outputFloatImage), renderState.w, renderState.h, type))
+
+    def RenderFreeView(self, camera, renderState, outputCharImage, outputFloatImage, type=abi.RENDER_SHADED_GREYSCALE, sync=True):
+        """b200_render_view_async: FindVisibleBlocks + CreateExpectedDepths + RenderImage(type) + RenderImage(RENDER_DEPTH_MAP) from
+        one pose as one enqueue and one raycast, into a free-view render state. Either image may be None. sync=False only
+        enqueues (renderState.noVisibleBlocks is then refreshed by RenderFreeViewSync)."""
+        self.e.after_torch()
+        self.e.check(self.e.lib.b200_render_view_async(self.e.h, C.byref(self.scene.c), C.byref(renderState.c), C.byref(camera), type,
+                                                        _ptr(outputCharImage), _ptr(outputFloatImage)))
+        if sync:
+            self.RenderFreeViewSync(renderState)
+
+    def RenderFreeViewSync(self, renderState):
+        self.e.check(self.e.lib.b200_render_view_sync(self.e.h, C.byref(renderState.c)))
+
+    def RenderFreeViewSubmit(self, camera, renderState, h_outChar, h_outFloat, type=abi.RENDER_SHADED_GREYSCALE, slot=0):
+        """b200_render_view_submit: the same render, the images landing in the host tensors h_outChar / h_outFloat (pinned or
+        pageable; either may be None) once RenderFreeViewWait(slot) returns."""
+        self.e.after_torch()
+        self.e.check(self.e.lib.b200_render_view_submit(self.e.h, C.byref(self.scene.c), C.byref(renderState.c), C.byref(camera), type,
+                                                         _ptr(h_outChar), _ptr(h_outFloat), slot))
+
+    def RenderFreeViewWait(self, slot):
+        self.e.check(self.e.lib.b200_render_view_wait(self.e.h, slot))
 
     def CreateICPMaps(self, view, renderState, points, normals):
         self.e.after_torch()

@@ -295,6 +295,21 @@ class ITMVisualisationEngine_B200<TVoxel, ITMVoxelBlockHash> : public ITMVisuali
                                (b200_render_type)type));
   }
 
+  // Not an ITMLib virtual: FindVisibleBlocks + CreateExpectedDepths + RenderImage(type) + RenderImage(RENDER_DEPTH_MAP) from one
+  // pose as one enqueue and one raycast (b200_render_view_async), then the wait that refreshes renderState->noVisibleBlocks.
+  // renderState is a free-view render state sized like the output images; either image may be NULL.
+  void RenderFreeView(const ITMPose *pose, const ITMIntrinsics *intrinsics, ITMRenderState *renderState, ITMUChar4Image *outputCharImage,
+                      ITMFloatImage *outputFloatImage, IITMVisualisationEngine::RenderImageType type) const {
+    b200_scene s = b200_detail::PackScene(mutableScene());
+    b200_render_state r = b200_detail::PackRenderState(renderState);
+    b200_camera c = b200_detail::PackCamera(pose, intrinsics);
+    h->check(b200_render_view_async(h->e, &s, &r, &c, (b200_render_type)type,
+                                    outputCharImage ? (b200_vec4u *)outputCharImage->GetData(MEMORYDEVICE_CUDA) : NULL,
+                                    outputFloatImage ? outputFloatImage->GetData(MEMORYDEVICE_CUDA) : NULL));
+    h->check(b200_render_view_sync(h->e, &r));
+    b200_detail::UnpackRenderState(r, renderState);
+  }
+
   void FindSurface(const ITMPose *pose, const ITMIntrinsics *intrinsics, const ITMRenderState *renderState) const override {
     b200_scene s = b200_detail::PackScene(mutableScene());
     b200_render_state r = b200_detail::PackRenderState((ITMRenderState *)renderState);

@@ -182,7 +182,14 @@ size_t b200_decayed_block_count(const b200_engine *e);
 
 /* ---- ITMVisualisationEngine ---------------------------------------------------------------- */
 
-/* FindVisibleBlocks — Vis_CUDA.cu:151-180 */
+/* FindVisibleBlocks — Vis_CUDA.cu:151-180.
+   Constraint on free-view use of this call (and of b200_expected_depths after it) beside the fused path: the list's length
+   goes through the engine's one device-side visible count, which is the LIVE render state's list length for the next fused
+   frame, and the call marks the host counters as current although it refreshes none of the scene's. So (1) with frames of
+   b200_process_frame_async / b200_host_frame_submit* outstanding, call b200_sync() first: without it the next frame re-marks
+   the wrong number of blocks and allocates from stale free-list counters (seen on an H100: hash table, voxels and lists all
+   differ from a run without the render); (2) after these calls do not call b200_sync() again before the next frame: it would
+   hand the free view's count to the live render state. b200_render_view_async has neither constraint. */
 b200_status b200_find_visible_blocks(b200_engine *e, const b200_scene *scene,
                                      b200_render_state *rs, const b200_camera *cam);
 /* CreateExpectedDepths — Vis_CUDA.cu:194-240 */
@@ -264,6 +271,55 @@ b200_status b200_host_frame_submit(b200_engine *e, b200_scene *scene, b200_rende
                                    const float *h_depth, const b200_vec4u *h_rgb, b200_vec4f *d_points, b200_vec4f *d_normals,
                                    const b200_frame_opts *opts, b200_vec4u *h_outImage, int slot);
 b200_status b200_host_frame_wait(b200_engine *e, int slot);
+
+/* ---- free-view preview (no reference twin: ITMMainEngine::GetImage's FREECAMERA branch, ITMMainEngine.cpp:231-278, which
+   DynSLAM runs twice per volume and preview, once for the RGBA image and once for the depth) -----------------------------
+   b200_render_view_async is FindVisibleBlocks + CreateExpectedDepths + RenderImage(type) + RenderImage(RENDER_DEPTH_MAP) from
+   one pose as one enqueue: four launches on e's stream (image reset, table sweep that lists, projects and rasterises, the
+   raycast, one shading pass with two outputs), no host synchronisation, one raycast.
+
+   rs is a free-view render state: never the live one of a volume that is being fused (rejected when the engine can tell).
+   The outputs have rs's size, img_w x img_h. d_outChar (RGBA8) receives `type`, which is any render type but
+   B200_RENDER_DEPTH_MAP; d_outDepth (f32) receives the depth map; either may be NULL, not both. RENDER_COLOUR_FROM_NORMAL
+   leaves the alpha of found pixels as it is in d_outChar, as RenderImage does.
+
+   Valid once the work has run (stream order on e's stream, or after b200_render_view_sync): rs->d_visibleBlockPositions,
+   rs->d_minmax (the whole image), rs->d_raycastResult, d_outChar and d_outDepth, byte for byte what b200_find_visible_blocks,
+   b200_expected_depths, b200_render_image(type) and b200_render_image(B200_RENDER_DEPTH_MAP) leave for the same scene, render
+   state and camera; the MAX_RENDERING_BLOCKS rule is decided on the device. rs->noVisibleBlocks is a host field: only
+   b200_render_view_sync refreshes it.
+
+   It reads the scene and writes rs's buffers, the outputs and scratch of its own: none of the volume's counters, nothing a
+   fused frame or a checkpoint reads. It may be enqueued with asynchronous frames outstanding, before or after them, any number
+   of times; the frames' results do not change. (It counts as launched work for b200_checkpoint_save's kept classification: a
+   save after it classifies afresh.)
+
+   B200_ERR_INVALID, before anything is allocated or enqueued: a scene that does not fit the engine, rs, one of the three
+   buffers named above or cam missing, a non-positive size, both outputs NULL, B200_RENDER_DEPTH_MAP or an unknown value as
+   type, the live render state of the last fused frame as rs. */
+b200_status b200_render_view_async(b200_engine *e, const b200_scene *scene, b200_render_state *rs, const b200_camera *cam,
+                                   b200_render_type type, b200_vec4u *d_outChar, float *d_outDepth);
+/* The host waits for e's stream and sets rs->noVisibleBlocks to the count of the latest b200_render_view_async, whose render
+   state rs must be (B200_ERR_INVALID otherwise). Touches no other host field: the volume's counters stay as b200_sync() or
+   the asynchronous frames left them. */
+b200_status b200_render_view_sync(b200_engine *e, b200_render_state *rs);
+
+/* The same render with the images landing in host memory (pinned, or pageable at the price cudaMemcpyAsync charges for it):
+   the render goes to staging inside the engine, then a device-to-host copy on a copy stream of the preview's own, so that
+   preview k's download runs under preview k+1's, or the next fused frame's, kernels. Only enqueues. slot in {0, 1}; a slot may
+   be resubmitted only after b200_render_view_wait(slot) (B200_ERR_INVALID otherwise, nothing enqueued), and these slots are
+   not b200_host_frame_submit's: neither blocks the other. h_outChar / h_outDepth: as d_outChar / d_outDepth above, valid when
+   b200_render_view_wait(slot) returns; the alpha RENDER_COLOUR_FROM_NORMAL leaves on found pixels is 0 here. rs's buffers are
+   valid in stream order as above. A larger image than the slots have held needs both slots waited for first. */
+b200_status b200_render_view_submit(b200_engine *e, const b200_scene *scene, b200_render_state *rs, const b200_camera *cam,
+                                    b200_render_type type, b200_vec4u *h_outChar, float *h_outDepth, int slot);
+b200_status b200_render_view_wait(b200_engine *e, int slot);   /* the host waits for slot's images; OK when nothing is in flight */
+
+/* e's stream waits, on the device, for everything enqueued so far on producer's stream (an event record and a
+   cudaStreamWaitEvent; the host does not wait). This is what lets one engine composite layers other engines rendered
+   (b200_composite_instances, b200_composite_depth) with no host synchronisation between the renders and the composite.
+   Engines on the same device or on peers. */
+b200_status b200_engine_wait_engine(b200_engine *e, b200_engine *producer);
 
 /* ---- view builder (SURVEY 8(f) rank 1): the step immediately before fusion ------------------------
    Replaces ITMViewBuilder_CUDA (Engine/DeviceSpecific/CUDA/ITMViewBuilder_CUDA.cu). All images are
