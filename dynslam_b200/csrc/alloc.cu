@@ -735,53 +735,6 @@ k_serve_list(const float *__restrict__ depth, b200_hash_entry *table, int numBuc
   }
 }
 
-// free-view visible list (FindVisibleBlocks, Vis_CUDA.cu:151-180, :536-569): every entry with ptr >= 0
-// that passes the frustum test, ascending entry order; the visibility bytes are not touched.
-#define FV_EPT 16
-#define FV_TILE (256 * FV_EPT)
-__global__ void __launch_bounds__(256, 4)
-k_freeview_list(const b200_hash_entry *__restrict__ table, int noTotal, b200_vec3i *visiblePos, int capacity, DevCounters *ctr,
-                unsigned long long *scanDesc, unsigned gen, Mat4 M, float p0, float p1, float p2, float p3, float voxelSize, int w, int h) {
-  __shared__ unsigned sm[33];
-  __shared__ unsigned tileBase;
-  const float proj[4] = {p0, p1, p2, p3};
-  const int noTiles = (noTotal + FV_TILE - 1) / FV_TILE;
-  for (int tile = blockIdx.x; tile < noTiles; tile += gridDim.x) {
-    // strided assignment inside the tile keeps the 20-byte entry reads of a warp adjacent
-    unsigned mask = 0;
-    for (int k = 0; k < FV_EPT; ++k) {
-      const int idx = tile * FV_TILE + k * 256 + threadIdx.x;
-      if (idx < noTotal) {
-        Entry en = load_entry(table, idx);
-        if (en.ptr >= 0 && block_visible(en.x, en.y, en.z, M, proj, voxelSize, w, h)) mask |= 1u << k;
-      }
-    }
-    // order inside the tile must be ascending entry index: rank = sum over k' < k of count(k') + rank within row k
-    unsigned total = 0;
-    unsigned offs[FV_EPT];
-#pragma unroll
-    for (int k = 0; k < FV_EPT; ++k) {
-      unsigned rowTotal;
-      const unsigned r = block_exclusive_scan((mask >> k) & 1u, sm, &rowTotal);
-      offs[k] = total + r;
-      total += rowTotal;
-    }
-    if (threadIdx.x < 32) {
-      const unsigned ex = scan_lookback(scanDesc, gen, tile, total);
-      if (threadIdx.x == 0) { tileBase = ex; if (tile == noTiles - 1) ctr->noVisibleBlocks = (int)(ex + total); }
-    }
-    __syncthreads();
-#pragma unroll
-    for (int k = 0; k < FV_EPT; ++k) if ((mask >> k) & 1u) {
-      const int idx = tile * FV_TILE + k * 256 + threadIdx.x;
-      const Entry en = load_entry(table, idx);
-      const unsigned o = tileBase + offs[k];
-      if ((int)o < capacity) { b200_vec3i p; p.x = en.x; p.y = en.y; p.z = en.z; visiblePos[o] = p; }
-    }
-    __syncthreads();
-  }
-}
-
 void launch_allocate(b200_engine *e, const SceneRef &s, const FrameGeom &g, const float *depth, bool onlyVisible, int frameIdx,
                      int snapSlot, b200_vec2f *minmaxFused, int mw, int mh) {
   cudaStream_t st = e->stream;
@@ -808,12 +761,4 @@ void launch_allocate(b200_engine *e, const SceneRef &s, const FrameGeom &g, cons
                                                               (unsigned)e->maxRenderingBlocks, e->traceOn ? e->d_dbg : nullptr);
   trace_end(e, st);
   e->launches += 2;
-}
-
-void launch_find_visible(b200_engine *e, const SceneRef &s, const Mat4 &M, const float proj[4], int w, int h, float voxelSize) {
-  const int noTiles = (s.noTotal + FV_TILE - 1) / FV_TILE;
-  k_freeview_list<<<persistent_grid(e, 4, noTiles), 256, 0, e->stream>>>(s.hash, s.noTotal, s.visiblePos, s.numBlocks, e->d_ctr,
-                                                                        e->d_scanDesc, ++e->scanGen, M, proj[0], proj[1], proj[2], proj[3],
-                                                                        voxelSize, w, h);
-  e->launches++;
 }

@@ -118,6 +118,8 @@ struct DevCounters {
   int droppedSnapshots;    // decay: snapshots found overwritten in the ring when their turn came (swept as empty)
   unsigned noRenderingBlocks;
   unsigned visCtasDone;    // k_serve_list: CTAs that have finished (the last one applies the rendering-block cap if needed)
+  unsigned depthCtasDone;  // k_expected_depths: the same for the stand-alone CreateExpectedDepths
+  unsigned listTicket;     // k_freeview_list: next table tile to hand out (reset by the launch's last draw)
   unsigned tilesRanked;    // k_serve_list: tiles that have published their request counts
   unsigned tilesListed;    // ... that have written their part of the visible list (the per-entry phase starts when all have)
   unsigned tilesWithExcess, tilesExcessServed;   // ... of which have excess-list requests / have served them (excess-part tiles list only after all have)
@@ -214,7 +216,7 @@ DEV void atomic_min_posf(float *a, float v) { atomicMin(reinterpret_cast<int *>(
 DEV void atomic_max_posf(float *a, float v) { atomicMax(reinterpret_cast<int *>(a), __float_as_int(v)); }
 
 // ------------------------------------------------------------------------------------------------
-// visibility test (DA/ITMSceneReconstructionEngine.h:315-397): alloc.cu's sweeps and the free-view preview (preview.cu)
+// visibility test (DA/ITMSceneReconstructionEngine.h:315-397): alloc.cu's sweeps and FindVisibleBlocks (vis.cu)
 // ------------------------------------------------------------------------------------------------
 DEV bool point_visible(const Mat4 &M, const float *proj, float x, float y, float z, int w, int h) {
   Vec4 b = m4v4(M, x, y, z, 1.0f);
@@ -240,7 +242,7 @@ __device__ inline bool block_visible(int bx, int by, int bz, const Mat4 &M, cons
 }
 
 // ------------------------------------------------------------------------------------------------
-// expected depths: block projection shared by vis.cu (k_project_blocks) and alloc.cu (k_visible_list)
+// expected depths: block projection shared by vis.cu (k_expected_depths) and alloc.cu (k_serve_list)
 // ------------------------------------------------------------------------------------------------
 // ProjectSingleBlock — DA/ITMVisualisationEngine.h:29-71
 DEV bool project_single_block(int bx, int by, int bz, const Mat4 &pose, const float *intr, int w, int h, float voxelSize,

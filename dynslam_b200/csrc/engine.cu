@@ -391,7 +391,8 @@ b200_status b200_find_visible_blocks(b200_engine *e, const b200_scene *s, b200_r
   CK(cudaSetDevice(e->device));
   st = upload(e, s, rs); if (st) return st;
   if (e->ptrListFor == (const void *)rs->d_visibleBlockPositions) e->ptrListFor = nullptr;   // list rebuilt without ptrs
-  launch_find_visible(e, scene_ref(s, rs), to_mat(cam->M), cam->proj, rs->img_w, rs->img_h, s->voxelSize);
+  launch_find_visible(e, scene_ref(s, rs), to_mat(cam->M), cam->proj, rs->img_w, rs->img_h, s->voxelSize, &e->d_ctr->noVisibleBlocks,
+                      &e->d_ctr->listTicket, e->d_scanDesc, ++e->scanGen);
   return download_sync(e, nullptr, rs);
 }
 
@@ -400,12 +401,8 @@ b200_status b200_expected_depths(b200_engine *e, const b200_scene *s, b200_rende
   CK(cudaSetDevice(e->device));
   st = upload(e, s, rs); if (st) return st;
   e->deadPending = false;      // the whole image is rebuilt here
-  // one pass with atomics; it counts the rendering tiles, and only if they break MAX_RENDERING_BLOCKS (whose rule depends on the
-  // list order) the ordered two-kernel form rebuilds the image
-  launch_expected_depths_fast(e, scene_ref(s, rs), to_mat(cam->M), cam->proj, rs->img_w, rs->img_h, s->voxelSize, rs->d_minmax);
-  st = download_sync(e, nullptr, nullptr); if (st) return st;
-  if (e->h_ctr->noRenderingBlocks <= (unsigned)e->maxRenderingBlocks) return B200_OK;
-  launch_expected_depths(e, scene_ref(s, rs), to_mat(cam->M), cam->proj, rs->img_w, rs->img_h, s->voxelSize, rs->d_minmax);
+  launch_expected_depths(e, scene_ref(s, rs), to_mat(cam->M), cam->proj, rs->img_w, rs->img_h, s->voxelSize, rs->d_minmax,
+                         &e->d_ctr->noVisibleBlocks, &e->d_ctr->noRenderingBlocks, &e->d_ctr->depthCtasDone);
   return download_sync(e, nullptr, nullptr);
 }
 
@@ -425,8 +422,9 @@ b200_status b200_render_image(b200_engine *e, const b200_scene *s, b200_render_s
   CK(cudaSetDevice(e->device));
   SceneRef r = scene_ref(s, rs);
   launch_raycast(e, r, to_mat(cam->invM), cam->proj, out_w, out_h, s->voxelSize, s->mu, rs->d_minmax, rs->d_raycastResult);
-  launch_shade(e, r, to_mat(cam->M), to_mat(cam->invM), out_w, out_h, s->voxelSize, s->maxW, rs->d_raycastResult, d_outChar, d_outFloat,
-               (int)type);
+  const bool depth = type == B200_RENDER_DEPTH_MAP;
+  launch_shade(e, r, to_mat(cam->M), to_mat(cam->invM), out_w, out_h, s->voxelSize, s->maxW, rs->d_raycastResult, depth ? nullptr : d_outChar,
+               depth ? d_outFloat : nullptr, (int)type);
   CK(cudaStreamSynchronize(e->stream));
   CK(cudaGetLastError());
   return B200_OK;
@@ -616,8 +614,7 @@ static b200_status frame_enqueue(b200_engine *e, b200_scene *s, b200_render_stat
     // bounds, so blocks along the right and bottom image borders smear over thousands of them: ~10^6 atomics, 38 us measured)
     // are read by nothing on the device. They are brought up to date when the host can next look at the image — b200_sync() —
     // from the block records of the latest frame, instead of every frame.
-    e->deadPending = true; e->deadScene = r; e->deadM = g.M_d; memcpy(e->deadProj, g.proj_d, sizeof(e->deadProj));
-    e->deadW = rs->img_w; e->deadH = rs->img_h; e->deadVoxelSize = s->voxelSize; e->deadMinmax = rs->d_minmax;
+    e->deadPending = true; e->deadScene = r; e->deadW = rs->img_w; e->deadH = rs->img_h; e->deadMinmax = rs->d_minmax;
   }
   launch_integrate(e, r, g, v->d_depth, v->d_rgb);
   if (e->evMid && !e->useGraph) { CK(cudaEventRecord(e->evMid, e->stream)); e->midValid = true; }
@@ -657,7 +654,7 @@ static b200_status frame_enqueue(b200_engine *e, b200_scene *s, b200_render_stat
 b200_status b200_sync(b200_engine *e, b200_scene *s, b200_render_state *rs) {
   CK(cudaSetDevice(e->device));
   if (e->deadPending) {      // see frame_enqueue: the part of the expected-depth image nothing on the device reads
-    launch_expected_depths_dead(e, e->deadScene, e->deadM, e->deadProj, e->deadW, e->deadH, e->deadVoxelSize, e->deadMinmax);
+    launch_expected_depths_dead(e, e->deadScene, e->deadW, e->deadH, e->deadMinmax);
     e->deadPending = false;
   }
   b200_status st = download_sync(e, s, rs); if (st) return st;

@@ -88,7 +88,7 @@ struct b200_engine {
   // timing mode 3: an event pair around every kernel launch (launch trace, b200_get_trace)
   bool traceOn; int traceCount, traceCap; cudaEvent_t *traceEv; const char **traceName;
   // expected-depth cells outside the live corner of the latest fused frame: rasterised lazily at b200_sync()
-  bool deadPending; SceneRef deadScene; Mat4 deadM; float deadProj[4]; int deadW, deadH; float deadVoxelSize; b200_vec2f *deadMinmax;
+  bool deadPending; SceneRef deadScene; int deadW, deadH; b200_vec2f *deadMinmax;
   unsigned long long *d_evalCounters, *h_evalCounters;   // evaluation consumer: counters (device) and their pinned mirror, allocated on first use
   unsigned long long *d_meshDesc;     // meshing: chained-scan descriptors, one per VBA block (allocated on first use)
   unsigned long long *d_dbg;          // timestamps written by instrumented kernels while the launch trace is on (b200_diag_read_debug)
@@ -142,17 +142,22 @@ static inline const int *fresh_ptr_list(const b200_engine *e, const SceneRef &s)
 }
 void launch_decay_partial(b200_engine *e, const SceneRef &s, int snapSlot, int minAge, int maxWeight, int frameIdx);
 void launch_decay_full(b200_engine *e, const SceneRef &s, int minAge, int maxWeight, int frameIdx);
-void launch_find_visible(b200_engine *e, const SceneRef &s, const Mat4 &M, const float proj[4], int w, int h, float voxelSize);
-void launch_expected_depths(b200_engine *e, const SceneRef &s, const Mat4 &M, const float proj[4], int w, int h,
-                            float voxelSize, b200_vec2f *minmax, bool deadInitDone = false, bool recsReady = false);
-void launch_expected_depths_fast(b200_engine *e, const SceneRef &s, const Mat4 &M, const float proj[4], int w, int h, float voxelSize,
-                                 b200_vec2f *minmax);
-void launch_expected_depths_dead(b200_engine *e, const SceneRef &s, const Mat4 &M, const float proj[4], int w, int h, float voxelSize,
-                                 b200_vec2f *minmax);
+// FindVisibleBlocks into s.visiblePos; the count, the tile ticket and the scan descriptors (FV_TILE entries per tile) are the
+// caller's, so that the free-view preview keeps its own
+#define FV_EPT 16
+#define FV_TILE (256 * FV_EPT)
+void launch_find_visible(b200_engine *e, const SceneRef &s, const Mat4 &M, const float proj[4], int w, int h, float voxelSize,
+                         int *count, unsigned *ticket, unsigned long long *scanDesc, unsigned gen);
+// CreateExpectedDepths over the first *count items of s.visiblePos; *tiles receives the rendering-tile total, *done is the
+// pass's self-resetting CTA counter
+void launch_expected_depths(b200_engine *e, const SceneRef &s, const Mat4 &M, const float proj[4], int w, int h, float voxelSize,
+                            b200_vec2f *minmax, const int *count, unsigned *tiles, unsigned *done);
+// the fused frame's expected-depth cells outside the live corner, from the block records of its allocation
+void launch_expected_depths_dead(b200_engine *e, const SceneRef &s, int w, int h, b200_vec2f *minmax);
 void launch_raycast(b200_engine *e, const SceneRef &s, const Mat4 &invM, const float proj[4], int w, int h, float voxelSize,
                     float mu, const b200_vec2f *minmax, b200_vec4f *out);
 void launch_shade(b200_engine *e, const SceneRef &s, const Mat4 &M, const Mat4 &invM, int w, int h, float voxelSize, int maxW,
-                  const b200_vec4f *rays, b200_vec4u *outChar, float *outFloat, int type);
+                  const b200_vec4f *rays, b200_vec4u *outChar, float *outDepth, int type);
 void launch_icp(b200_engine *e, const Mat4 &invM, int w, int h, float voxelSize, const b200_vec4f *rays, b200_vec4u *outImg,
                 b200_vec4f *points, b200_vec4f *normals);
 void launch_forward_render(b200_engine *e, const SceneRef &s, const FrameGeom &g, const float *depth, const b200_vec2f *minmax,

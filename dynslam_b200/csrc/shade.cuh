@@ -1,5 +1,5 @@
-// shade.cuh — per-pixel shading from the volume, shared by k_shade (vis.cu) and the free-view preview's k_preview_shade
-// (preview.cu): the SDF normal, the interpolated colour and the RGBA pixel of every RenderImage type but the depth map.
+// shade.cuh — per-pixel shading from the volume for k_shade (vis.cu): the SDF normal, the interpolated colour, the RGBA pixel
+// of every RenderImage type but the depth map, and the depth pixel.
 #pragma once
 #include "raycast_ray.cuh"
 

@@ -1,211 +1,132 @@
-// vis.cu — ITMVisualisationEngine for sm_90a: expected depths, hierarchical raycast, shading,
-// ICP maps, forward render, point cloud.
+// vis.cu — ITMVisualisationEngine for sm_90a: visible list, expected depths, hierarchical raycast, shading, ICP maps,
+// forward render, point cloud.
 //
-// Replaces (reference ITMVisualisationEngine_CUDA.cu): memsetKernel + projectAndSplitBlocks_device +
-// fillBlocks_device (:194-240, :572-637), genericRaycast_device (:672-684) with castRay
-// (DeviceAgnostic/ITMVisualisationEngine.h:93-179), the five render*_device kernels (:735-886),
-// renderICP_device (:716-724), forwardProject/findMissingPoints/genericRaycastMissingPoints/
-// renderForward (:639-733) and renderPointCloud_device (:820-871).
+// Replaces (reference ITMVisualisationEngine_CUDA.cu): buildVisibleList_device (:151-180, :536-569), memsetKernel +
+// projectAndSplitBlocks_device + fillBlocks_device (:194-240, :572-637), genericRaycast_device (:672-684) with castRay
+// (DeviceAgnostic/ITMVisualisationEngine.h:93-179), the five render*_device kernels (:735-886), renderICP_device (:716-724),
+// forwardProject/findMissingPoints/genericRaycastMissingPoints/renderForward (:639-733) and renderPointCloud_device (:820-871).
 //
 // Differences in shape: no materialised RenderingBlock list and no blocking copy of its length —
 // each visible block rasterises its own bounding box into the 1/8-resolution min/max image with
-// native integer atomics on the (positive) float bit patterns, the MAX_RENDERING_BLOCKS rule is
-// applied from a list-order prefix of the tile counts; rays are traced by 8x4-pixel warps so that
-// a warp's rays walk the same voxel blocks; the voxel reads fetch the 2-byte sdf only.
+// native integer atomics on the (positive) float bit patterns, and the MAX_RENDERING_BLOCKS rule is
+// applied on the device by the CTA that finishes last, only when the tile total breaks it; rays are
+// traced by 8x4-pixel warps so that a warp's rays walk the same voxel blocks; the voxel reads fetch
+// the 2-byte sdf only.
 #include "engine.h"
 #include "raycast_ray.cuh"
 #include "shade.cuh"
 #include <cstdlib>
 
 // ------------------------------------------------------------------------------------------------
-// expected depths
+// visible list
 // ------------------------------------------------------------------------------------------------
-// ProjectSingleBlock (DA/ITMVisualisationEngine.h:29-71) and the 16-byte block record live in common.cuh: the visible-list
-// pass of the fused frame (alloc.cu) produces the records too.
-// Stage 1: project every visible block (one thread each, small CTAs so that a few thousand blocks spread over
-// many SMs), apply the MAX_RENDERING_BLOCKS rule from the list-order prefix of the tile counts (Vis_CUDA.cu:609)
-// and emit a 16-byte record {bbox, z-range}. Cells of a bounding box that lie outside the live 1/8-resolution
-// corner (the reference clamps boxes to the FULL-resolution bounds, DA/ITMVisualisationEngine.h:57-60) are
-// rasterised here with global atomics; they are rare and never read by the raycast.
-// Stage 2 (k_fill_minmax): the live corner is cut into 8x8-cell tiles, one CTA per tile; the CTA scans all
-// records, rasterises the boxes that overlap its tile into shared memory with shared-memory atomics and
-// writes the tile out with plain stores — no global atomics on the hot cells that hundreds of far blocks
-// cover, and no separate initialisation of the live corner.
-
-#define PRJ_THREADS 128   // small CTAs: they must fit beside the integrate kernel's CTAs (register file)
-__global__ void __launch_bounds__(PRJ_THREADS)
-k_project_blocks(const b200_hash_entry *__restrict__ table, int numBuckets, const b200_vec3i *__restrict__ visiblePos,
-                 const int *__restrict__ visiblePtr, int capacity, DevCounters *ctr, Mat4 M, float p0, float p1, float p2, float p3, int w,
-                 int h, float voxelSize, float2 *minmax, BlockRec *recs, unsigned long long *scanDesc, unsigned gen, int recsReady, unsigned maxRB) {
+// FindVisibleBlocks: every entry with ptr >= 0 that passes the frustum test, ascending entry order; the visibility bytes are
+// not touched. *count receives the number found, not capped by the list's capacity (the reference's count is not either).
+// Tiles are handed out through a ticket, not by blockIdx: a tile then only ever waits for tiles whose CTAs are already
+// running, so the chained scan's look-back cannot stall when the grid is not co-resident (two engines' sweeps sharing the
+// GPU). Every CTA draws exactly one ticket past the last tile, so ticket noTiles + gridDim.x - 1 is the launch's last draw and
+// the CTA that draws it resets the ticket for the next launch.
+__global__ void __launch_bounds__(256, 4)
+k_freeview_list(const b200_hash_entry *__restrict__ table, int noTotal, b200_vec3i *visiblePos, int capacity, int *count,
+                unsigned *ticket, unsigned long long *scanDesc, unsigned gen, Mat4 M, float p0, float p1, float p2, float p3,
+                float voxelSize, int w, int h) {
   __shared__ unsigned sm[33];
   __shared__ unsigned tileBase;
-  const float intr[4] = {p0, p1, p2, p3};
-  int n = ctr->noVisibleBlocks;
-  if (n > capacity) n = capacity;
-  const int noTiles = (n + PRJ_THREADS - 1) / PRJ_THREADS;
-  const int liveX = (w - 1) / B200_MINMAX_SUBSAMPLE, liveY = (h - 1) / B200_MINMAX_SUBSAMPLE;   // last live cell
-  const int lane = threadIdx.x & 31;
-  // Fused frame (recsReady): k_serve_list (alloc.cu) already wrote the records, cap rule included, and rasterised the live corner; what is left is
-  // the dead-cell part of the boxes, which nothing in the frame reads (a block next to the camera can cover 10^5 of them), so
-  // it runs AFTER the fill the raycast waits for. Stand-alone CreateExpectedDepths (recsReady 0) does everything here.
-  const bool fast = recsReady != 0;
-  const bool doDead = true;
-  for (int tile = blockIdx.x; tile < noTiles; tile += gridDim.x) {
-    const int item = tile * PRJ_THREADS + threadIdx.x;
-    int ulx = 0, uly = 0, lrx = -1, lry = -1; float zmin = 0, zmax = 0;
-    unsigned required = 0;
-    bool draw;
-    if (fast) {
-      if (item < n) {
-        const uint4 q = __ldg(reinterpret_cast<const uint4 *>(recs) + item);
-        ulx = (short)(q.x & 0xffff); uly = (short)(q.x >> 16); lrx = (short)(q.y & 0xffff); lry = (short)(q.y >> 16);
-        zmin = __uint_as_float(q.z); zmax = __uint_as_float(q.w);
-      }
-      draw = ulx <= lrx;
-    } else {
-    if (item < n) {
-      const b200_vec3i p = visiblePos[item];
-      const bool allocated = visiblePtr ? (visiblePtr[item] >= 0) : (find_block<false>(table, numBuckets, p.x, p.y, p.z) >= 0);
-      if (allocated) {
-        if (project_single_block(p.x, p.y, p.z, M, intr, w, h, voxelSize, ulx, uly, lrx, lry, zmin, zmax)) {
-          required = rendering_tiles(ulx, uly, lrx, lry);
-        }
+  __shared__ int sTile;
+  const float proj[4] = {p0, p1, p2, p3};
+  const int noTiles = (noTotal + FV_TILE - 1) / FV_TILE;
+  for (;;) {
+    if (threadIdx.x == 0) {
+      const unsigned t = atomicAdd(ticket, 1u);
+      if (t == (unsigned)noTiles + gridDim.x - 1) *ticket = 0;
+      sTile = (int)t;
+    }
+    __syncthreads();
+    const int tile = sTile;
+    if (tile >= noTiles) break;
+    // strided assignment inside the tile keeps the 20-byte entry reads of a warp adjacent
+    unsigned mask = 0;
+    for (int k = 0; k < FV_EPT; ++k) {
+      const int idx = tile * FV_TILE + k * 256 + threadIdx.x;
+      if (idx < noTotal) {
+        Entry en = load_entry(table, idx);
+        if (en.ptr >= 0 && block_visible(en.x, en.y, en.z, M, proj, voxelSize, w, h)) mask |= 1u << k;
       }
     }
-    unsigned total;
-    const unsigned local = block_exclusive_scan(required, sm, &total);
+    // order inside the tile must be ascending entry index: rank = sum over k' < k of count(k') + rank within row k
+    unsigned total = 0;
+    unsigned offs[FV_EPT];
+#pragma unroll
+    for (int k = 0; k < FV_EPT; ++k) {
+      unsigned rowTotal;
+      const unsigned r = block_exclusive_scan((mask >> k) & 1u, sm, &rowTotal);
+      offs[k] = total + r;
+      total += rowTotal;
+    }
     if (threadIdx.x < 32) {
       const unsigned ex = scan_lookback(scanDesc, gen, tile, total);
-      if (threadIdx.x == 0) { tileBase = ex; if (tile == noTiles - 1) ctr->noRenderingBlocks = ex + total; }
+      if (threadIdx.x == 0) { tileBase = ex; if (tile == noTiles - 1) *count = (int)(ex + total); }
     }
     __syncthreads();
-    const unsigned out_offset = tileBase + local;
-    draw = required > 0 && (out_offset + required <= maxRB);   // :609
-    if (item < n) {
-      BlockRec r;
-      if (draw) { r.ulx = (short)ulx; r.uly = (short)uly; r.lrx = (short)lrx; r.lry = (short)lry; r.zmin = zmin; r.zmax = zmax; }
-      else { r.ulx = 1; r.uly = 1; r.lrx = 0; r.lry = 0; r.zmin = 0; r.zmax = 0; }
-      recs[item] = r;
-    }
-    }
-    // the part of a box outside the live corner (dead cells): warp-cooperative, one box at a time
-    unsigned todo = __ballot_sync(0xffffffffu, doDead && item < n && draw && (lrx > liveX || lry > liveY));
-    while (todo) {
-      const int src = __ffs(todo) - 1;
-      todo &= todo - 1;
-      const int ax = __shfl_sync(0xffffffffu, ulx, src), ay = __shfl_sync(0xffffffffu, uly, src);
-      const int bx = __shfl_sync(0xffffffffu, lrx, src), by = __shfl_sync(0xffffffffu, lry, src);
-      const float zn = __shfl_sync(0xffffffffu, zmin, src), zx = __shfl_sync(0xffffffffu, zmax, src);
-      const int bw = bx - ax + 1, cnt = bw * (by - ay + 1);
-      for (int k = lane; k < cnt; k += 32) {
-        const int yy = ay + k / bw, xx = ax + k % bw;
-        if (xx > liveX || yy > liveY) { float2 *px = &minmax[xx + yy * w]; atomic_min_posf(&px->x, zn); atomic_max_posf(&px->y, zx); }
-      }
+#pragma unroll
+    for (int k = 0; k < FV_EPT; ++k) if ((mask >> k) & 1u) {
+      const int idx = tile * FV_TILE + k * 256 + threadIdx.x;
+      const Entry en = load_entry(table, idx);
+      const unsigned o = tileBase + offs[k];
+      if ((int)o < capacity) { b200_vec3i p; p.x = en.x; p.y = en.y; p.z = en.z; visiblePos[o] = p; }
     }
     __syncthreads();
   }
-  if (!fast && noTiles == 0 && blockIdx.x == 0 && threadIdx.x == 0) ctr->noRenderingBlocks = 0;
 }
 
-#define FILL_T 8          // tile edge in 1/8-resolution cells
-#define FILL_THREADS 128
-__global__ void __launch_bounds__(FILL_THREADS)
-k_fill_minmax(const BlockRec *__restrict__ recs, const DevCounters *ctr, int capacity, int w, int h, float2 *minmax) {
-  __shared__ int smin[FILL_T * FILL_T], smax[FILL_T * FILL_T];
-  const int liveX = (w - 1) / B200_MINMAX_SUBSAMPLE, liveY = (h - 1) / B200_MINMAX_SUBSAMPLE;
-  const int tx0 = blockIdx.x * FILL_T, ty0 = blockIdx.y * FILL_T;
-  const int tx1 = min(tx0 + FILL_T - 1, liveX), ty1 = min(ty0 + FILL_T - 1, liveY);
-  if (threadIdx.x < FILL_T * FILL_T) { smin[threadIdx.x] = __float_as_int(B200_FAR_AWAY); smax[threadIdx.x] = __float_as_int(B200_VERY_CLOSE); }
-  __syncthreads();
-  int n = ctr->noVisibleBlocks;
-  if (n > capacity) n = capacity;
-  const uint4 *r4 = reinterpret_cast<const uint4 *>(recs);
-  for (int i0 = threadIdx.x; i0 < n; i0 += FILL_THREADS * 8) {
-    uint4 q8[8];
-#pragma unroll
-    for (int u = 0; u < 8; ++u) { const int i = i0 + u * FILL_THREADS; q8[u] = (i < n) ? __ldg(r4 + i) : make_uint4(1u | (1u << 16), 0u, 0u, 0u); }   // 8 loads in flight
-#pragma unroll
-    for (int u = 0; u < 8; ++u) {
-      const uint4 q = q8[u];
-      const int ulx = (short)(q.x & 0xffff), uly = (short)(q.x >> 16), lrx = (short)(q.y & 0xffff), lry = (short)(q.y >> 16);
-      const int ax = max(ulx, tx0), bx = min(lrx, tx1), ay = max(uly, ty0), by = min(lry, ty1);
-      if (ax > bx || ay > by) continue;
-      const int zn = (int)q.z, zx = (int)q.w;   // positive floats: integer order == float order
-      for (int yy = ay; yy <= by; ++yy)
-        for (int xx = ax; xx <= bx; ++xx) {
-          const int c = (yy - ty0) * FILL_T + (xx - tx0);
-          atomicMin(&smin[c], zn);
-          atomicMax(&smax[c], zx);
-        }
-    }
-  }
-  __syncthreads();
-  if (threadIdx.x < FILL_T * FILL_T) {
-    const int xx = tx0 + (threadIdx.x % FILL_T), yy = ty0 + (threadIdx.x / FILL_T);
-    if (xx <= tx1 && yy <= ty1) minmax[xx + yy * w] = make_float2(__int_as_float(smin[threadIdx.x]), __int_as_float(smax[threadIdx.x]));
-  }
-}
-
-// initialises every cell OUTSIDE the live corner (the live corner is written in full by k_fill_minmax)
-__global__ void k_minmax_init_dead(float2 *minmax, int w, int h) {
-  const int liveX = (w - 1) / B200_MINMAX_SUBSAMPLE, liveY = (h - 1) / B200_MINMAX_SUBSAMPLE;
-  const float2 v = make_float2(B200_FAR_AWAY, B200_VERY_CLOSE);
-  const int n = w * h;
-  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
-    const int y = i / w, x = i - y * w;
-    if (x > liveX || y > liveY) minmax[i] = v;
-  }
-}
-
-void launch_expected_depths(b200_engine *e, const SceneRef &s, const Mat4 &M, const float proj[4], int w, int h, float voxelSize,
-                            b200_vec2f *minmax, bool deadInitDone, bool recsReady) {
-  if (!deadInitDone) { k_minmax_init_dead<<<e->smCount * 4, 256, 0, e->stream>>>((float2 *)minmax, w, h); e->launches++; }
-  const int noTiles = (s.numBlocks + PRJ_THREADS - 1) / PRJ_THREADS;
-  if (!recsReady) {   // otherwise the records come from k_serve_list of this frame; the dead cells follow in launch_expected_depths_dead
-    trace_begin(e, e->stream, "k_project_blocks");
-    k_project_blocks<<<persistent_grid(e, 2, noTiles), PRJ_THREADS, 0, e->stream>>>(s.hash, s.numBuckets, s.visiblePos, fresh_ptr_list(e, s),
-                                                                                   s.numBlocks, e->d_ctr, M, proj[0], proj[1], proj[2], proj[3],
-                                                                                   w, h, voxelSize, (float2 *)minmax, (BlockRec *)e->d_blockRecs,
-                                                                                   e->d_scanDesc, ++e->scanGen, 0, (unsigned)e->maxRenderingBlocks);
-    trace_end(e, e->stream);
-    e->launches++;
-  }
-  dim3 grid(((w - 1) / B200_MINMAX_SUBSAMPLE) / FILL_T + 1, ((h - 1) / B200_MINMAX_SUBSAMPLE) / FILL_T + 1);
-  trace_begin(e, e->stream, "k_fill_minmax");
-  k_fill_minmax<<<grid, FILL_THREADS, 0, e->stream>>>((const BlockRec *)e->d_blockRecs, e->d_ctr, s.numBlocks, w, h, (float2 *)minmax);
+void launch_find_visible(b200_engine *e, const SceneRef &s, const Mat4 &M, const float proj[4], int w, int h, float voxelSize,
+                         int *count, unsigned *ticket, unsigned long long *scanDesc, unsigned gen) {
+  const int noTiles = (s.noTotal + FV_TILE - 1) / FV_TILE;
+  trace_begin(e, e->stream, "k_freeview_list");
+  k_freeview_list<<<persistent_grid(e, 4, noTiles), 256, 0, e->stream>>>(s.hash, s.noTotal, s.visiblePos, s.numBlocks, count, ticket,
+                                                                        scanDesc, gen, M, proj[0], proj[1], proj[2], proj[3], voxelSize,
+                                                                        w, h);
   trace_end(e, e->stream);
-  e->launches += 1;
+  e->launches++;
 }
 
-// ---- stand-alone CreateExpectedDepths, fast form ------------------------------------------------------------------------
-// One pass over the visible list: every listed block goes to an 8-lane group (a corner per lane, project_block_group), its box
-// — clamped to the FULL-resolution bounds, as the reference does — is rasterised with atomic min / max into the image that
-// k_minmax_init_all reset: by the group up to 64 cells, by the warp up to 512, by the whole CTA beyond (the boxes of blocks
-// that leave the frustum on the right or at the bottom spill over up to 10^5 cells of the part of the image nothing reads).
-// The MAX_RENDERING_BLOCKS rule is order dependent; this pass only COUNTS the rendering tiles, and when the total breaks the cap
-// (never at KITTI sizes) the host runs the ordered two-kernel form above instead (engine.cu).
-#define XD_BIG 64
-__global__ void k_minmax_init_all(float2 *minmax, int n, DevCounters *ctr) {
-  if (blockIdx.x == 0 && threadIdx.x == 0) ctr->noRenderingBlocks = 0;
+// ------------------------------------------------------------------------------------------------
+// expected depths
+// ------------------------------------------------------------------------------------------------
+// ProjectSingleBlock (DA/ITMVisualisationEngine.h:29-71), its 8-lane form, the box rasterisers and the 16-byte block record
+// live in common.cuh: the visible-list pass of the fused frame (alloc.cu) uses them too.
+__global__ void k_minmax_reset(float2 *minmax, int n, unsigned *tiles) {
+  if (blockIdx.x == 0 && threadIdx.x == 0) *tiles = 0;
   const float2 v = make_float2(B200_FAR_AWAY, B200_VERY_CLOSE);
   for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) minmax[i] = v;
 }
 
+// CreateExpectedDepths over a visible list, into the image k_minmax_reset has reset. Every listed block goes to an 8-lane
+// group (a corner per lane, project_block_group); its box — clamped to the FULL-resolution bounds, as the reference does — is
+// rasterised with atomic min / max: by the group up to 64 cells, by the warp up to 512, by the whole CTA beyond (the boxes of
+// blocks that leave the frustum on the right or at the bottom spill over up to 10^5 cells of the part of the image nothing
+// reads). The rendering tiles of the drawn boxes are summed into *tiles.
+// The MAX_RENDERING_BLOCKS rule (Vis_CUDA.cu:609: a block is dropped when the running tile count in list order would pass the
+// cap) depends on the order, so every box is drawn first; the CTA that finishes last (*done counts them and is reset by it)
+// knows the total, and only if that breaks the cap (never at KITTI sizes) does it reset the image and walk the list in order,
+// re-projecting every block and drawing the ones the rule keeps. Every other CTA has finished, so their atomics are all in.
+#define XD_BIG 64
 __global__ void __launch_bounds__(256)
-k_expected_depths_fast(const b200_hash_entry *__restrict__ table, int numBuckets, const b200_vec3i *__restrict__ visiblePos,
-                       const int *__restrict__ visiblePtr, int capacity, DevCounters *ctr, Mat4 M, float p0, float p1, float p2, float p3, int w,
-                       int h, float voxelSize, float2 *minmax) {
+k_expected_depths(const b200_hash_entry *__restrict__ table, int numBuckets, const b200_vec3i *__restrict__ visiblePos,
+                  const int *__restrict__ visiblePtr, int capacity, const int *count, unsigned *tiles, unsigned *done, Mat4 M, float p0,
+                  float p1, float p2, float p3, int w, int h, float voxelSize, float2 *minmax, unsigned maxRB) {
   __shared__ BlockRec bigRecs[XD_BIG];
   __shared__ int bigCount;
+  __shared__ unsigned sm[33];
+  __shared__ bool lastCta;
   const float intr[4] = {p0, p1, p2, p3};
   const int lane = threadIdx.x & 31, grp = threadIdx.x >> 3, sub = threadIdx.x & 7;
   if (threadIdx.x == 0) bigCount = 0;
   __syncthreads();
-  int n = ctr->noVisibleBlocks;
+  int n = *count;
   if (n > capacity) n = capacity;
-  unsigned myTiles = 0;
-  for (int i0 = blockIdx.x * 32; i0 < n; i0 += gridDim.x * 32) {
-    const int item = i0 + grp;
+  // the box of list item `item` for the calling 8-lane group (all 32 lanes call it); false: not drawn
+  auto item_box = [&](int item, int &ulx, int &uly, int &lrx, int &lry, float &zl, float &zh) {
     bool have = false;
     int ex = 0, ey = 0, ez = 0;
     if (item < n) {
@@ -213,8 +134,12 @@ k_expected_depths_fast(const b200_hash_entry *__restrict__ table, int numBuckets
       ex = p.x; ey = p.y; ez = p.z;
       have = visiblePtr ? (__ldg(visiblePtr + item) >= 0) : (find_block<false>(table, numBuckets, p.x, p.y, p.z) >= 0);
     }
+    return project_block_group(have, ex, ey, ez, M, intr, w, h, voxelSize, ulx, uly, lrx, lry, zl, zh);
+  };
+  unsigned myTiles = 0;
+  for (int i0 = blockIdx.x * 32; i0 < n; i0 += gridDim.x * 32) {
     int ulx, uly, lrx, lry; float zl, zh;
-    const bool draw = project_block_group(have, ex, ey, ez, M, intr, w, h, voxelSize, ulx, uly, lrx, lry, zl, zh);
+    const bool draw = item_box(i0 + grp, ulx, uly, lrx, lry, zl, zh);
     if (draw && sub == 0) myTiles += rendering_tiles(ulx, uly, lrx, lry);
     const int cells = draw ? (lrx - ulx + 1) * (lry - uly + 1) : 0;
     if (cells > 0 && cells <= 64) raster_box_group(minmax, w, ulx, uly, lrx, lry, zl, zh);
@@ -238,7 +163,7 @@ k_expected_depths_fast(const b200_hash_entry *__restrict__ table, int numBuckets
     }
   }
   for (int o = 16; o > 0; o >>= 1) myTiles += __shfl_xor_sync(0xffffffffu, myTiles, o);
-  if (lane == 0 && myTiles) atomicAdd(&ctr->noRenderingBlocks, myTiles);
+  if (lane == 0 && myTiles) atomicAdd(tiles, myTiles);
   __syncthreads();
   const int nb = bigCount < XD_BIG ? bigCount : XD_BIG;
   for (int b = 0; b < nb; ++b) {
@@ -251,29 +176,91 @@ k_expected_depths_fast(const b200_hash_entry *__restrict__ table, int numBuckets
         atomic_min_posf(&px->x, br.zmin); atomic_max_posf(&px->y, br.zmax);
       }
   }
+  // ---------------- tail: the CTA that finishes last owns the cap rule ----------------
+  __threadfence();
+  __syncthreads();
+  if (threadIdx.x == 0) lastCta = (atomicAdd(done, 1u) == gridDim.x - 1);
+  __syncthreads();
+  if (!lastCta) return;
+  if (threadIdx.x == 0) *done = 0;
+  if (*(volatile unsigned *)tiles <= maxRB) return;
+  for (int i = threadIdx.x; i < w * h; i += blockDim.x) minmax[i] = make_float2(B200_FAR_AWAY, B200_VERY_CLOSE);
+  __syncthreads();
+  unsigned running = 0;
+  for (int base = 0; base < n; base += 32) {     // 32 items per round, in list order over the groups
+    int ulx, uly, lrx, lry; float zl, zh;
+    const bool draw = item_box(base + grp, ulx, uly, lrx, lry, zl, zh);
+    const unsigned required = (draw && sub == 0) ? rendering_tiles(ulx, uly, lrx, lry) : 0u;
+    unsigned total;
+    const unsigned before = running + block_exclusive_scan(required, sm, &total);
+    running += total;
+    unsigned todo = __ballot_sync(0xffffffffu, required > 0 && before + required <= maxRB);   // :609
+    while (todo) {
+      const int src = __ffs(todo) - 1;
+      todo &= todo - 1;
+      const int ax = __shfl_sync(0xffffffffu, ulx, src), ay = __shfl_sync(0xffffffffu, uly, src);
+      const int bx = __shfl_sync(0xffffffffu, lrx, src), by = __shfl_sync(0xffffffffu, lry, src);
+      const float zn = __shfl_sync(0xffffffffu, zl, src), zx = __shfl_sync(0xffffffffu, zh, src);
+      raster_box_warp(minmax, w, ax, ay, bx, by, zn, zx);
+    }
+  }
 }
 
-void launch_expected_depths_fast(b200_engine *e, const SceneRef &s, const Mat4 &M, const float proj[4], int w, int h, float voxelSize,
-                                 b200_vec2f *minmax) {
-  k_minmax_init_all<<<e->smCount * 4, 256, 0, e->stream>>>((float2 *)minmax, w * h, e->d_ctr);
+// reset + list pass; *count is the list's length as the sweep that built it counted it
+void launch_expected_depths(b200_engine *e, const SceneRef &s, const Mat4 &M, const float proj[4], int w, int h, float voxelSize,
+                            b200_vec2f *minmax, const int *count, unsigned *tiles, unsigned *done) {
+  k_minmax_reset<<<e->smCount * 4, 256, 0, e->stream>>>((float2 *)minmax, w * h, tiles);
   const int groupsOf32 = (s.numBlocks + 31) / 32;
-  trace_begin(e, e->stream, "k_expected_depths_fast");
-  k_expected_depths_fast<<<persistent_grid(e, 4, groupsOf32), 256, 0, e->stream>>>(s.hash, s.numBuckets, s.visiblePos, fresh_ptr_list(e, s), s.numBlocks,
-                                                                                  e->d_ctr, M, proj[0], proj[1], proj[2], proj[3], w, h, voxelSize,
-                                                                                  (float2 *)minmax);
+  trace_begin(e, e->stream, "k_expected_depths");
+  k_expected_depths<<<persistent_grid(e, 4, groupsOf32), 256, 0, e->stream>>>(s.hash, s.numBuckets, s.visiblePos, fresh_ptr_list(e, s),
+                                                                              s.numBlocks, count, tiles, done, M, proj[0], proj[1], proj[2],
+                                                                              proj[3], w, h, voxelSize, (float2 *)minmax,
+                                                                              (unsigned)e->maxRenderingBlocks);
   trace_end(e, e->stream);
   e->launches += 2;
 }
 
-// second half of the fused frame's expected-depth work: the dead cells (after launch_expected_depths(..., recsReady = true))
-void launch_expected_depths_dead(b200_engine *e, const SceneRef &s, const Mat4 &M, const float proj[4], int w, int h, float voxelSize,
-                                 b200_vec2f *minmax) {
-  const int noTiles = (s.numBlocks + PRJ_THREADS - 1) / PRJ_THREADS;
-  trace_begin(e, e->stream, "k_project_blocks/dead");
-  k_project_blocks<<<persistent_grid(e, 2, noTiles), PRJ_THREADS, 0, e->stream>>>(s.hash, s.numBuckets, s.visiblePos, fresh_ptr_list(e, s),
-                                                                                 s.numBlocks, e->d_ctr, M, proj[0], proj[1], proj[2], proj[3],
-                                                                                 w, h, voxelSize, (float2 *)minmax, (BlockRec *)e->d_blockRecs,
-                                                                                 e->d_scanDesc, ++e->scanGen, 2, (unsigned)e->maxRenderingBlocks);
+// The cells of the fused frame's expected-depth image outside the live 1/8-resolution corner. k_serve_list (alloc.cu) wrote the
+// block records, cap rule included, and rasterised the live corner; the rest of the boxes is read by nothing in the frame (a
+// block next to the camera can cover 10^5 of those cells), so it is drawn from the records when the host can next see the
+// image (b200_sync, engine.cu): one record per thread, the boxes that reach outside the corner one at a time per warp.
+#define DEAD_THREADS 128   // small CTAs: they must fit beside the integrate kernel's CTAs (register file)
+__global__ void __launch_bounds__(DEAD_THREADS)
+k_dead_cells(const BlockRec *__restrict__ recs, const DevCounters *ctr, int capacity, int w, int h, float2 *minmax) {
+  const int liveX = (w - 1) / B200_MINMAX_SUBSAMPLE, liveY = (h - 1) / B200_MINMAX_SUBSAMPLE;   // last live cell
+  const int lane = threadIdx.x & 31;
+  int n = ctr->noVisibleBlocks;
+  if (n > capacity) n = capacity;
+  const int noTiles = (n + DEAD_THREADS - 1) / DEAD_THREADS;
+  for (int tile = blockIdx.x; tile < noTiles; tile += gridDim.x) {
+    const int item = tile * DEAD_THREADS + threadIdx.x;
+    int ulx = 0, uly = 0, lrx = -1, lry = -1; float zmin = 0, zmax = 0;
+    if (item < n) {
+      const uint4 q = __ldg(reinterpret_cast<const uint4 *>(recs) + item);
+      ulx = (short)(q.x & 0xffff); uly = (short)(q.x >> 16); lrx = (short)(q.y & 0xffff); lry = (short)(q.y >> 16);
+      zmin = __uint_as_float(q.z); zmax = __uint_as_float(q.w);
+    }
+    unsigned todo = __ballot_sync(0xffffffffu, ulx <= lrx && (lrx > liveX || lry > liveY));
+    while (todo) {
+      const int src = __ffs(todo) - 1;
+      todo &= todo - 1;
+      const int ax = __shfl_sync(0xffffffffu, ulx, src), ay = __shfl_sync(0xffffffffu, uly, src);
+      const int bx = __shfl_sync(0xffffffffu, lrx, src), by = __shfl_sync(0xffffffffu, lry, src);
+      const float zn = __shfl_sync(0xffffffffu, zmin, src), zx = __shfl_sync(0xffffffffu, zmax, src);
+      const int bw = bx - ax + 1, cnt = bw * (by - ay + 1);
+      for (int k = lane; k < cnt; k += 32) {
+        const int yy = ay + k / bw, xx = ax + k % bw;
+        if (xx > liveX || yy > liveY) { float2 *px = &minmax[xx + yy * w]; atomic_min_posf(&px->x, zn); atomic_max_posf(&px->y, zx); }
+      }
+    }
+  }
+}
+
+void launch_expected_depths_dead(b200_engine *e, const SceneRef &s, int w, int h, b200_vec2f *minmax) {
+  const int noTiles = (s.numBlocks + DEAD_THREADS - 1) / DEAD_THREADS;
+  trace_begin(e, e->stream, "k_dead_cells");
+  k_dead_cells<<<persistent_grid(e, 2, noTiles), DEAD_THREADS, 0, e->stream>>>((const BlockRec *)e->d_blockRecs, e->d_ctr, s.numBlocks, w, h,
+                                                                              (float2 *)minmax);
   trace_end(e, e->stream);
   e->launches++;
 }
@@ -349,10 +336,12 @@ void launch_raycast(b200_engine *e, const SceneRef &s, const Mat4 &invM, const f
 // ------------------------------------------------------------------------------------------------
 // shading from the volume
 // ------------------------------------------------------------------------------------------------
-// RenderImage_common kernels — Vis_CUDA.cu:735-886; the per-pixel functions are in shade.cuh.
+// RenderImage_common kernels — Vis_CUDA.cu:735-886; the per-pixel functions are in shade.cuh. Two outputs, either may be null:
+// the RGBA pixel of `type` and the depth pixel (drawPixelDepth), so that the free-view preview gets both from one read of the
+// ray point.
 __global__ void __launch_bounds__(256)
 k_shade(const float4 *__restrict__ rays, const b200_voxel *__restrict__ voxels, const b200_hash_entry *__restrict__ table, int nb, int w, int h,
-        Mat4 M, float lx, float ly, float lz, float voxelSize, int maxW, uchar4 *outChar, float *outFloat, int type) {
+        Mat4 M, float lx, float ly, float lz, float voxelSize, int maxW, uchar4 *outChar, float *outDepth, int type) {
   const int tilesX = (w + 7) >> 3, tilesY = (h + 3) >> 2;
   const int warpGlobal = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
   if (warpGlobal >= tilesX * tilesY) return;
@@ -362,15 +351,18 @@ k_shade(const float4 *__restrict__ rays, const b200_voxel *__restrict__ voxels, 
   const int locId = x + y * w;
   const float4 pr = rays[locId];
   const bool found = pr.w > 0;
-  if (type == B200_RENDER_DEPTH_MAP) outFloat[locId] = depth_px(found, pr, M, voxelSize);
-  else shade_rgba_px(type, found, pr, voxels, table, nb, lx, ly, lz, maxW, &outChar[locId]);
+  if (outDepth) outDepth[locId] = depth_px(found, pr, M, voxelSize);
+  if (outChar) shade_rgba_px(type, found, pr, voxels, table, nb, lx, ly, lz, maxW, &outChar[locId]);
 }
 
+// either output may be null; `type` is the RGBA type outChar is shaded with
 void launch_shade(b200_engine *e, const SceneRef &s, const Mat4 &M, const Mat4 &invM, int w, int h, float voxelSize, int maxW,
-                  const b200_vec4f *rays, b200_vec4u *outChar, float *outFloat, int type) {
+                  const b200_vec4f *rays, b200_vec4u *outChar, float *outDepth, int type) {
   const int tiles = ((w + 7) / 8) * ((h + 3) / 4);
+  trace_begin(e, e->stream, "k_shade");
   k_shade<<<(tiles + 7) / 8, 256, 0, e->stream>>>((const float4 *)rays, s.voxels, s.hash, s.numBuckets, w, h, M, -invM.m[8], -invM.m[9],
-                                                 -invM.m[10], voxelSize, maxW, (uchar4 *)outChar, outFloat, type);
+                                                 -invM.m[10], voxelSize, maxW, (uchar4 *)outChar, outDepth, type);
+  trace_end(e, e->stream);
   e->launches++;
 }
 

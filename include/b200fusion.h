@@ -275,8 +275,9 @@ b200_status b200_host_frame_wait(b200_engine *e, int slot);
 /* ---- free-view preview (no reference twin: ITMMainEngine::GetImage's FREECAMERA branch, ITMMainEngine.cpp:231-278, which
    DynSLAM runs twice per volume and preview, once for the RGBA image and once for the depth) -----------------------------
    b200_render_view_async is FindVisibleBlocks + CreateExpectedDepths + RenderImage(type) + RenderImage(RENDER_DEPTH_MAP) from
-   one pose as one enqueue: four launches on e's stream (image reset, table sweep that lists, projects and rasterises, the
-   raycast, one shading pass with two outputs), no host synchronisation, one raycast.
+   one pose as one enqueue: five launches on e's stream, the kernels of the stand-alone calls (table sweep that lists, image
+   reset, one pass over the list that projects and rasterises, the raycast, one shading pass with two outputs), no host
+   synchronisation, one raycast.
 
    rs is a free-view render state: never the live one of a volume that is being fused (rejected when the engine can tell).
    The outputs have rs's size, img_w x img_h. d_outChar (RGBA8) receives `type`, which is any render type but

@@ -36,8 +36,8 @@ W, H = synth.KITTI_W, synth.KITTI_H
 DECAY = (1, 200)
 GEOMETRY = (0x60000, 0x100000, 0x80000)
 COLOUR = abi.RENDER_COLOUR_FROM_VOLUME
-# host synchronisations per preview, read from the code: each of the three synchronous calls ends in one stream synchronise
-# (b200_expected_depths in a second one only when the tile cap is broken), and each pageable cudaMemcpy blocks: 2 x (3 + 1);
+# host synchronisations per preview, read from the code: each of the three synchronous calls ends in one stream synchronise,
+# and each pageable cudaMemcpy blocks: 2 x (3 + 1);
 # the fused arm blocks once, in b200_render_view_wait
 HOST_SYNCS_READ_FROM_CODE = dict(reference_shape=8, fused=1)
 
