@@ -114,7 +114,11 @@ __global__ void __launch_bounds__(256)
 k_mark_prepare(const float *__restrict__ depth, const b200_hash_entry *__restrict__ table, int numBuckets,
                const b200_vec3i *__restrict__ prevList, uint8_t *visType, DevCounters *ctr, unsigned long long *reqKey, unsigned *reqBits,
                unsigned *req2Bits, uint8_t *markBytes, const __grid_constant__ FrameGeom g, unsigned frameTag, int capacity, int prepCtas,
-               float2 *minmax, int mw, int mh, unsigned tilesXMagic) {
+               float2 *minmax, int mw, int mh, unsigned tilesXMagic, unsigned long long *span) {
+  // First kernel of the chain, launched without the programmatic attribute: everything before it has completed, so the list
+  // kernel's CTAs may take the SM slots of this grid's retiring CTAs at once (they wait for its completion before any access).
+  pdl_trigger();
+  SpanStamp stamp(span);
   if ((int)blockIdx.x < prepCtas) {
     // ---- prepare part ----
     const int tid = blockIdx.x * blockDim.x + threadIdx.x, nth = prepCtas * blockDim.x;
@@ -332,7 +336,8 @@ k_serve_list(const float *__restrict__ depth, b200_hash_entry *table, int numBuc
              const int *__restrict__ allocList, const int *__restrict__ excessList, DevCounters *ctr, const __grid_constant__ FrameGeom g,
              int currentFrame, int onlyVisible, unsigned long long *descA, unsigned long long *descB, unsigned long long *descC,
              unsigned gen, b200_vec3i *visiblePos, int *visiblePtr, int capacity, b200_vec3i *ring, long long ringCap, long long *snapStart,
-             int *snapCount, int slot, BlockRec *recs, float2 *minmax, int rw, int rh, unsigned maxRB, unsigned long long *dbg) {
+             int *snapCount, int slot, BlockRec *recs, float2 *minmax, int rw, int rh, unsigned maxRB, unsigned long long *dbg,
+             unsigned long long *span) {
   __shared__ unsigned sm[33];
   __shared__ unsigned tileBase, tileBase2;
   __shared__ BlockRec bigRecs[AL_BIG];
@@ -342,6 +347,8 @@ k_serve_list(const float *__restrict__ depth, b200_hash_entry *table, int numBuc
 #define K2_TILE_STAMP(k, tile) do { if (dbg && threadIdx.x == 0 && (tile) < 1024) { unsigned long long t_; asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t_)); dbg[64 + (k) * 1024 + (tile)] = t_; } } while (0)
 #define K2_SUB(j, cond) do { if (dbgSlot >= 0 && threadIdx.x == 0 && (cond)) { unsigned long long t_; asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t_)); dbg[32 + dbgSlot * 8 + (j)] = t_; } } while (0)
 #define K2_STAMP(i) do { if (dbgSlot >= 0 && threadIdx.x == 0) { unsigned long long t_; asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t_)); dbg[dbgSlot * 8 + (i)] = t_; } } while (0)
+  pdl_wait();            // everything below reads k_mark_prepare's requests and marks
+  SpanStamp stamp(span);
   K2_STAMP(0);
   const int noWords = noTotal >> 5;
   const int noTiles = (noTotal + AL_TILE - 1) / AL_TILE;
@@ -679,6 +686,7 @@ k_serve_list(const float *__restrict__ depth, b200_hash_entry *table, int numBuc
       }
     }
   }
+  pdl_trigger();         // this CTA has no list work left: the integrate kernel's CTAs may take its SM slots as it retires
   // ---------------- tail: the CTA that finishes last resets the per-launch counters and owns the cap rule ----------------
   if (recs) {
     for (int o = 16; o > 0; o >>= 1) myTiles += __shfl_xor_sync(0xffffffffu, myTiles, o);
@@ -736,7 +744,7 @@ k_serve_list(const float *__restrict__ depth, b200_hash_entry *table, int numBuc
 }
 
 void launch_allocate(b200_engine *e, const SceneRef &s, const FrameGeom &g, const float *depth, bool onlyVisible, int frameIdx,
-                     int snapSlot, b200_vec2f *minmaxFused, int mw, int mh) {
+                     int snapSlot, b200_vec2f *minmaxFused, int mw, int mh, bool fused) {
   cudaStream_t st = e->stream;
   const unsigned frameTag = (unsigned)(frameIdx + 1) & 0xffffffu;
   if (frameTag == 0) cudaMemsetAsync(e->d_reqKey, 0, sizeof(unsigned long long) * (size_t)s.noTotal, st);
@@ -746,19 +754,20 @@ void launch_allocate(b200_engine *e, const SceneRef &s, const FrameGeom &g, cons
   k_mark_prepare<<<prepCtas + (tiles + 7) / 8, 256, 0, st>>>(depth, s.hash, s.numBuckets, s.visiblePos, s.visType, e->d_ctr, e->d_reqKey,
                                                             e->d_reqBits, e->d_req2Bits, e->d_markBytes, g, frameTag, s.numBlocks, prepCtas,
                                                             (float2 *)minmaxFused, mw, mh,
-                                                            (unsigned)((0x100000000ull + (unsigned)((g.w + 7) / 8) - 1) / (unsigned)((g.w + 7) / 8)));
+                                                            (unsigned)((0x100000000ull + (unsigned)((g.w + 7) / 8) - 1) / (unsigned)((g.w + 7) / 8)),
+                                                            fused ? span_slot(e, SPAN_MARK) : nullptr);
   trace_end(e, st);
   const int noTiles = (s.noTotal + AL_TILE - 1) / AL_TILE;
   const unsigned gen = ++e->scanGen;
   const int third = e->scanDescCap / 3;
   trace_begin(e, st, "k_serve_list");
-  k_serve_list<<<persistent_grid(e, 2, noTiles), 256, 0, st>>>(depth, s.hash, s.numBuckets, s.noTotal, s.visType, e->d_reqKey, e->d_reqBits,
-                                                              e->d_req2Bits, e->d_markBytes, s.allocationList, s.excessList, e->d_ctr, g,
-                                                              frameIdx, onlyVisible ? 1 : 0, e->d_scanDesc, e->d_scanDesc + third,
-                                                              e->d_scanDesc + 2 * third, gen, s.visiblePos, e->d_visiblePtr, s.numBlocks,
-                                                              e->d_ring, e->ringCap, e->d_snapStart, e->d_snapCount, snapSlot,
-                                                              minmaxFused ? (BlockRec *)e->d_blockRecs : nullptr, (float2 *)minmaxFused, mw, mh,
-                                                              (unsigned)e->maxRenderingBlocks, e->traceOn ? e->d_dbg : nullptr);
+  // chained in every caller: the list kernel always directly follows the marking kernel
+  launch_chained(true, k_serve_list, persistent_grid(e, 2, noTiles), 256, 0, st, depth, s.hash, s.numBuckets, s.noTotal, s.visType,
+                 e->d_reqKey, e->d_reqBits, e->d_req2Bits, e->d_markBytes, s.allocationList, s.excessList, e->d_ctr, g, frameIdx,
+                 onlyVisible ? 1 : 0, e->d_scanDesc, e->d_scanDesc + third, e->d_scanDesc + 2 * third, gen, s.visiblePos, e->d_visiblePtr,
+                 s.numBlocks, e->d_ring, e->ringCap, e->d_snapStart, e->d_snapCount, snapSlot,
+                 minmaxFused ? (BlockRec *)e->d_blockRecs : nullptr, (float2 *)minmaxFused, mw, mh, (unsigned)e->maxRenderingBlocks,
+                 e->traceOn ? e->d_dbg : nullptr, fused ? span_slot(e, SPAN_SERVE) : nullptr);
   trace_end(e, st);
   e->launches += 2;
 }

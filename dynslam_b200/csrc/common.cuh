@@ -211,6 +211,27 @@ DEV void st_stream(uint4 *p, uint4 v) {
   asm volatile("st.global.L1::no_allocate.v4.u32 [%0], {%1,%2,%3,%4};" ::"l"(p), "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w) : "memory");
 }
 
+// Programmatic dependent launch (Hopper griddepcontrol). The rules every kernel of the fused frame's chain keeps are written at
+// launch_chained (engine.h). In a grid launched without the programmatic attribute both instructions are no-ops.
+DEV void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
+DEV void pdl_trigger() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
+
+DEV unsigned long long global_timer() { unsigned long long t; asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t)); return t; }
+
+// Span of one launch in %globaltimer nanoseconds (b200_set_timing modes 2 and 4): span[0] = ~(earliest stamp at a CTA's entry,
+// taken after its pdl_wait), span[1] = latest stamp at a warp's exit. The complement lets one zero-filled slot take both as
+// atomicMax. span == nullptr: nothing is stamped. Constructed by thread 0 of a CTA for the entry; destroyed by every thread,
+// lane 0 of each warp stamps when its warp leaves the scope (early returns included).
+struct SpanStamp {
+  unsigned long long *span;
+  DEV explicit SpanStamp(unsigned long long *s) : span(s) {
+    if (span && threadIdx.x == 0) atomicMax(span, ~global_timer());
+  }
+  DEV ~SpanStamp() {
+    if (span && (threadIdx.x & 31) == 0) atomicMax(span + 1, global_timer());
+  }
+};
+
 // positive-float atomic min/max through the order-preserving int view (all values here are > 0)
 DEV void atomic_min_posf(float *a, float v) { atomicMin(reinterpret_cast<int *>(a), __float_as_int(v)); }
 DEV void atomic_max_posf(float *a, float v) { atomicMax(reinterpret_cast<int *>(a), __float_as_int(v)); }

@@ -32,7 +32,10 @@ __global__ void __launch_bounds__(256)
 k_decay_blocks(b200_voxel *voxels, const b200_hash_entry *table, int numBuckets, const b200_vec3i *ring,
                long long ringCap, const long long *snapStart, const int *snapCount, int slot, const short4 *allocatedPos,
                int numBlocks, int minAge, int maxWeight, int currentFrame, unsigned gen, unsigned long long *delTag,
-               int *itemPtr, DevCounters *ctr, int *candList, uint8_t *visType, int *allocList, int *delList, uint8_t *isLeader) {
+               int *itemPtr, DevCounters *ctr, int *candList, uint8_t *visType, int *allocList, int *delList, uint8_t *isLeader,
+               unsigned long long *span) {
+  pdl_wait();            // in the fused frame: the raycast reads the voxels and entries this sweep resets and unlinks
+  SpanStamp stamp(span);
   // One WARP per list item (a block = 256 uint4 = 8 per lane, all 8 loads in flight), 8 items per CTA: the per-item chain of
   // dependent loads (ring position -> hash chain -> voxels) overlaps across warps, so the few thousand items of a frame are
   // one wave of warps instead of ~5 sequential items per CTA.
@@ -361,21 +364,23 @@ void launch_push_snapshot(b200_engine *e, const b200_vec3i *positions, int n, in
 }
 
 static void decay_common(b200_engine *e, const SceneRef &s, int mode, int slot, int minAge, int maxWeight, int frameIdx,
-                         long long items) {
+                         long long items, bool fused = false) {
   cudaStream_t st = e->stream;
   const unsigned gen = ++e->decayGen;
   const int grid1 = persistent_grid(e, 6, (items + 7) / 8);   // 8 items (warps) per CTA
   if (mode == 0) {
     trace_begin(e, st, "k_decay_blocks<0>");
-    k_decay_blocks<0><<<grid1, 256, 0, st>>>(s.voxels, s.hash, s.numBuckets, e->d_ring, e->ringCap, e->d_snapStart, e->d_snapCount,
-                                            slot, e->d_allocatedPos, s.numBlocks, minAge, maxWeight, frameIdx, gen, e->d_delTag,
-                                            e->d_itemPtr, e->d_ctr, e->d_candList, s.visType, s.allocationList, e->d_delList, e->d_isLeader);
+    launch_chained(fused, k_decay_blocks<0>, grid1, 256, 0, st, s.voxels, s.hash, s.numBuckets, e->d_ring, e->ringCap, e->d_snapStart,
+                   e->d_snapCount, slot, e->d_allocatedPos, s.numBlocks, minAge, maxWeight, frameIdx, gen, e->d_delTag, e->d_itemPtr,
+                   e->d_ctr, e->d_candList, s.visType, s.allocationList, e->d_delList, e->d_isLeader,
+                   fused ? span_slot(e, SPAN_DECAY) : nullptr);
     trace_end(e, st);
   } else {
     trace_begin(e, st, "k_decay_blocks<1>");
     k_decay_blocks<1><<<grid1, 256, 0, st>>>(s.voxels, s.hash, s.numBuckets, e->d_ring, e->ringCap, e->d_snapStart, e->d_snapCount,
                                             slot, e->d_allocatedPos, s.numBlocks, minAge, maxWeight, frameIdx, gen, e->d_delTag,
-                                            e->d_itemPtr, e->d_ctr, e->d_candList, s.visType, s.allocationList, e->d_delList, e->d_isLeader);
+                                            e->d_itemPtr, e->d_ctr, e->d_candList, s.visType, s.allocationList, e->d_delList, e->d_isLeader,
+                                            nullptr);
     trace_end(e, st);
   }
   if (mode == 0) { e->launches += 1; return; }   // the sweep's last CTA has committed the pass
@@ -390,9 +395,9 @@ static void decay_common(b200_engine *e, const SceneRef &s, int mode, int slot, 
   e->launches += 5;
 }
 
-void launch_decay_partial(b200_engine *e, const SceneRef &s, int snapSlot, int minAge, int maxWeight, int frameIdx) {
+void launch_decay_partial(b200_engine *e, const SceneRef &s, int snapSlot, int minAge, int maxWeight, int frameIdx, bool fused) {
   // item count lives on the device (snapCount[slot]); size the grid for the capacity
-  decay_common(e, s, 0, snapSlot, minAge, maxWeight, frameIdx, s.numBlocks);
+  decay_common(e, s, 0, snapSlot, minAge, maxWeight, frameIdx, s.numBlocks, fused);
 }
 
 void launch_decay_full(b200_engine *e, const SceneRef &s, int minAge, int maxWeight, int frameIdx) {

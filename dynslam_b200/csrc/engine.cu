@@ -225,7 +225,7 @@ void b200_engine_destroy(b200_engine *e) {
   }
   if (e->frameGraph) cudaGraphExecDestroy(e->frameGraph);
   if (e->sideStream) { cudaStreamSynchronize(e->sideStream); if (e->evFork) cudaEventDestroy(e->evFork); if (e->evJoin) cudaEventDestroy(e->evJoin); cudaStreamDestroy(e->sideStream); }
-  if (e->evRing) { for (int i = 0; i < e->evRingCap * 2; ++i) cudaEventDestroy(e->evRing[i]); free(e->evRing); }
+  cudaFree(e->d_spans);
   if (e->traceEv) { for (int i = 0; i < e->traceCap * 2; ++i) cudaEventDestroy(e->traceEv[i]); free(e->traceEv); free(e->traceName); }
   cudaGetLastError();
   checkpoint_release(e);
@@ -240,11 +240,12 @@ int32_t b200_frame_index(const b200_engine *e) { return e->frameIdx; }
 size_t b200_decayed_block_count(const b200_engine *e) { return (size_t)e->totalDecayed; }
 void b200_set_timing(b200_engine *e, int mode) {
   e->timing = mode != 0;
-  e->evRingCount = 0;
-  if (mode >= 2 && !e->evRing) {
-    e->evRingCap = 8192;
-    e->evRing = (cudaEvent_t *)calloc((size_t)e->evRingCap * 2, sizeof(cudaEvent_t));
-    for (int i = 0; i < e->evRingCap * 2; ++i) cudaEventCreate(&e->evRing[i]);
+  e->spanCount = 0;
+  if (mode >= 2) {
+    cudaSetDevice(e->device);
+    const size_t bytes = sizeof(unsigned long long) * 2 * SPAN_KERNELS * SPAN_FRAMES;
+    if (!e->d_spans && cudaMalloc(&e->d_spans, bytes) != cudaSuccess) { cudaGetLastError(); e->d_spans = nullptr; }
+    if (e->d_spans) cudaMemsetAsync(e->d_spans, 0, bytes, e->stream);   // behind any frame still stamping the old records
   }
   e->timingMode = mode;
   e->traceOn = mode == 3;
@@ -282,6 +283,19 @@ void b200_diag_last_integrate(const b200_engine *e, int *kernel, int *grid) {
   if (grid) *grid = e->lastIntegrateGrid;
 }
 
+int b200_diag_read_spans(b200_engine *e, unsigned long long *out, int maxFrames) {
+  if (!e || !out || maxFrames <= 0 || !e->d_spans || e->timingMode < 2) return 0;
+  const int n = e->spanCount < maxFrames ? e->spanCount : maxFrames;
+  if (n == 0) return 0;
+  cudaSetDevice(e->device);
+  const size_t words = (size_t)n * SPAN_KERNELS * 2;
+  if (cudaMemcpyAsync(out, e->d_spans, sizeof(unsigned long long) * words, cudaMemcpyDeviceToHost, e->stream) != cudaSuccess ||
+      cudaStreamSynchronize(e->stream) != cudaSuccess)
+    return 0;
+  for (size_t i = 0; i < words; i += 2) out[i] = out[i] ? ~out[i] : 0;   // the entry stamp is kept complemented (SpanStamp)
+  return n;
+}
+
 int b200_diag_read_debug(b200_engine *e, unsigned long long *out, int n) {
   if (!e || !out || n <= 0) return 0;
   if (n > B200_DBG_WORDS) n = B200_DBG_WORDS;
@@ -316,7 +330,7 @@ int push_snapshot_slot(b200_engine *e) {
 }
 
 static b200_status enqueue_allocate(b200_engine *e, b200_scene *s, b200_render_state *rs, const b200_view *v, int onlyVisible,
-                                    bool fuseDeadInit = false) {
+                                    bool fuseDeadInit = false, bool fused = false) {
   if (v->depth_w != e->img_w || v->depth_h != e->img_h) {
     snprintf(e->err, sizeof(e->err), "view size %dx%d differs from engine %dx%d", v->depth_w, v->depth_h, e->img_w, e->img_h);
     return B200_ERR_INVALID;
@@ -324,7 +338,7 @@ static b200_status enqueue_allocate(b200_engine *e, b200_scene *s, b200_render_s
   const int slot = push_snapshot_slot(e);
   e->tableVersion++;
   launch_allocate(e, scene_ref(s, rs), frame_geom(s, v), v->d_depth, onlyVisible != 0, e->frameIdx, slot,
-                  fuseDeadInit ? rs->d_minmax : nullptr, rs->img_w, rs->img_h);
+                  fuseDeadInit ? rs->d_minmax : nullptr, rs->img_w, rs->img_h, fused);
   e->ptrListFor = rs->d_visibleBlockPositions; e->ptrListVersion = e->tableVersion;
   e->frameIdx++;
   return B200_OK;
@@ -365,14 +379,15 @@ b200_status b200_integrate(b200_engine *e, b200_scene *s, b200_render_state *rs,
   return download_sync(e, s, rs);
 }
 
-static void enqueue_decay(b200_engine *e, b200_scene *s, b200_render_state *rs, int maxWeight, int minAge, int forceAll) {
+static void enqueue_decay(b200_engine *e, b200_scene *s, b200_render_state *rs, int maxWeight, int minAge, int forceAll,
+                          bool fused = false) {
   SceneRef r = scene_ref(s, rs);
   e->tableVersion++;
   if (forceAll) launch_decay_full(e, r, minAge, maxWeight, e->frameIdx);
   else if ((long)e->qSize > minAge) {
     const int slot = e->qHead % SNAP_SLOTS;
     e->qHead++; e->qSize--;
-    launch_decay_partial(e, r, slot, minAge, maxWeight, e->frameIdx);
+    launch_decay_partial(e, r, slot, minAge, maxWeight, e->frameIdx, fused);
   }
 }
 
@@ -596,14 +611,15 @@ b200_status b200_process_frame_async(b200_engine *e, b200_scene *s, b200_render_
 static b200_status frame_enqueue(b200_engine *e, b200_scene *s, b200_render_state *rs, const b200_view *v, b200_vec4f *d_points,
                                  b200_vec4f *d_normals, const b200_frame_opts *opts) {
   b200_status st;
+  // The main-stream kernels are chained by programmatic dependent launch (launch_chained, engine.h): no stream operation may
+  // sit between them. The per-stage events of timing modes 1 and 3 do, and serialise the chain again; they are diagnostics.
+  const bool stages = e->timing && (e->timingMode == 1 || e->timingMode == 3);
   if (e->timing) CK(cudaEventRecord(e->ev[0], e->stream));
   const bool doRay = (!opts || opts->doRaycast);
-  st = enqueue_allocate(e, s, rs, v, 0, doRay); if (st) return st;
-  if (e->timing) CK(cudaEventRecord(e->ev[1], e->stream));
+  st = enqueue_allocate(e, s, rs, v, 0, doRay, true); if (st) return st;
+  if (stages) CK(cudaEventRecord(e->ev[1], e->stream));
   SceneRef r = scene_ref(s, rs);
   FrameGeom g = frame_geom(s, v);
-  const bool ring = e->timingMode >= 2 && e->evRingCount < e->evRingCap;
-  if (ring) CK(cudaEventRecord(e->evRing[2 * e->evRingCount], e->stream));
   // The expected-depth image of the live 1/8-resolution corner was rasterised by the allocation's list pass (alloc.cu),
   // MAX_RENDERING_BLOCKS rule included. Fork: what is left — the cells outside the corner, which nothing in the frame reads —
   // runs on the side stream underneath the integrate kernel.
@@ -616,13 +632,15 @@ static b200_status frame_enqueue(b200_engine *e, b200_scene *s, b200_render_stat
     // from the block records of the latest frame, instead of every frame.
     e->deadPending = true; e->deadScene = r; e->deadW = rs->img_w; e->deadH = rs->img_h; e->deadMinmax = rs->d_minmax;
   }
-  launch_integrate(e, r, g, v->d_depth, v->d_rgb);
+  launch_integrate(e, r, g, v->d_depth, v->d_rgb, true);
+  // evMid holds the pipelined upload of the next frame (host_frame_submit) back until the allocation and the integration are
+  // through. It splits the chain between the integrate kernel and the raycast on that path only; recorded behind the raycast
+  // instead, the upload lands under the next frame's allocation pair and the pipelined frame rate drops by about 15 % on the H100.
   if (e->evMid && !e->useGraph) { CK(cudaEventRecord(e->evMid, e->stream)); e->midValid = true; }
-  if (ring) { CK(cudaEventRecord(e->evRing[2 * e->evRingCount + 1], e->stream)); e->evRingCount++; }
-  if (e->timing) CK(cudaEventRecord(e->ev[2], e->stream));
+  if (stages) CK(cudaEventRecord(e->ev[2], e->stream));
   if (doRay) {
-    if (e->timing) CK(cudaEventRecord(e->ev[3], e->stream));
-    launch_raycast(e, r, g.invM_d, g.proj_d, rs->img_w, rs->img_h, s->voxelSize, s->mu, rs->d_minmax, rs->d_raycastResult);
+    if (stages) CK(cudaEventRecord(e->ev[3], e->stream));
+    launch_raycast(e, r, g.invM_d, g.proj_d, rs->img_w, rs->img_h, s->voxelSize, s->mu, rs->d_minmax, rs->d_raycastResult, true);
     // optional colour render for compositing: reads voxel colours, so it has to run before this frame's decay resets any
     if (opts && opts->d_colourRender)
       launch_shade(e, r, g.M_d, g.invM_d, rs->img_w, rs->img_h, s->voxelSize, s->maxW, rs->d_raycastResult, opts->d_colourRender, nullptr,
@@ -643,11 +661,12 @@ static b200_status frame_enqueue(b200_engine *e, b200_scene *s, b200_render_stat
         launch_shade(e, r, g.M_d, g.invM_d, rs->img_w, rs->img_h, s->voxelSize, s->maxW, rs->d_raycastResult, nullptr, opts->d_depthRender,
                      B200_RENDER_DEPTH_MAP);
     }
-  } else if (e->timing) CK(cudaEventRecord(e->ev[3], e->stream));
-  if (e->timing) CK(cudaEventRecord(e->ev[4], e->stream));
-  if (opts && opts->doDecay) enqueue_decay(e, s, rs, opts->decayMaxWeight, opts->decayMinAge, 0);
+  } else if (stages) CK(cudaEventRecord(e->ev[3], e->stream));
+  if (stages) CK(cudaEventRecord(e->ev[4], e->stream));
+  if (opts && opts->doDecay) enqueue_decay(e, s, rs, opts->decayMaxWeight, opts->decayMinAge, 0, true);
   if (overlap) CK(cudaStreamWaitEvent(mainStream, e->evJoin, 0));   // join: the frame is complete on the main stream
   if (e->timing) CK(cudaEventRecord(e->ev[5], e->stream));
+  if (e->timingMode >= 2 && e->d_spans && e->spanCount < SPAN_FRAMES) e->spanCount++;
   return B200_OK;
 }
 
@@ -969,20 +988,30 @@ b200_status b200_get_stats(b200_engine *e, b200_frame_stats *out) {
   out->noIntegratedBlocks = e->h_ctr->noIntegrated;
   out->totalIntegratedBlocks = e->h_ctr->totalIntegrated;
   out->droppedSnapshots = e->droppedSnapshots + e->h_ctr->droppedSnapshots;
-  if (e->timingMode >= 2 && e->evRingCount > 0) {
-    CK(cudaEventSynchronize(e->evRing[2 * e->evRingCount - 1]));
-    float sum = 0;
-    for (int i = 0; i < e->evRingCount; ++i) { float ms = 0; cudaEventElapsedTime(&ms, e->evRing[2 * i], e->evRing[2 * i + 1]); sum += ms; }
-    out->ring_ms_integrate = sum; out->ring_count = e->evRingCount;
+  if (e->timingMode >= 2 && e->spanCount > 0) {
+    // integrate launch durations from the kernels' own %globaltimer stamps: first CTA past its wait to the last warp's exit
+    const int n = e->spanCount;
+    unsigned long long *h = (unsigned long long *)malloc(sizeof(unsigned long long) * 2 * SPAN_KERNELS * (size_t)n);
+    if (!h) { snprintf(e->err, sizeof(e->err), "out of host memory"); return B200_ERR_INVALID; }
+    if (b200_diag_read_spans(e, h, n) != n) { free(h); snprintf(e->err, sizeof(e->err), "reading the kernel spans failed"); return B200_ERR_CUDA; }
+    double ns = 0; int count = 0;
+    for (int f = 0; f < n; ++f) {
+      const unsigned long long *sp = h + ((size_t)f * SPAN_KERNELS + SPAN_INTEGRATE) * 2;
+      if (sp[0] && sp[1] > sp[0]) { ns += (double)(sp[1] - sp[0]); count++; }
+    }
+    free(h);
+    out->ring_ms_integrate = (float)(ns * 1e-6); out->ring_count = count;
   }
   if (e->timing && e->timingMode != 0 && e->frameIdx > 0) {
     CK(cudaEventSynchronize(e->ev[5]));
-    cudaEventElapsedTime(&out->ms_allocate, e->ev[0], e->ev[1]);
-    cudaEventElapsedTime(&out->ms_integrate, e->ev[1], e->ev[2]);
-    cudaEventElapsedTime(&out->ms_expected, e->ev[2], e->ev[3]);
-    cudaEventElapsedTime(&out->ms_raycast, e->ev[3], e->ev[4]);
-    cudaEventElapsedTime(&out->ms_decay, e->ev[4], e->ev[5]);
     cudaEventElapsedTime(&out->ms_total, e->ev[0], e->ev[5]);
+    if (e->timingMode == 1 || e->timingMode == 3) {   // the stage events (frame_enqueue)
+      cudaEventElapsedTime(&out->ms_allocate, e->ev[0], e->ev[1]);
+      cudaEventElapsedTime(&out->ms_integrate, e->ev[1], e->ev[2]);
+      cudaEventElapsedTime(&out->ms_expected, e->ev[2], e->ev[3]);
+      cudaEventElapsedTime(&out->ms_raycast, e->ev[3], e->ev[4]);
+      cudaEventElapsedTime(&out->ms_decay, e->ev[4], e->ev[5]);
+    }
   }
   return B200_OK;
 }

@@ -2,6 +2,8 @@
 #pragma once
 #include "common.cuh"
 
+#include <utility>
+
 struct FrameGeom {          // per-call constants handed to kernels by value
   Mat4 M_d, invM_d, M_rgb;
   float proj_d[4], proj_rgb[4];
@@ -83,8 +85,8 @@ struct b200_engine {
   int useGraph; bool graphWarm; cudaGraphExec_t frameGraph;
   cudaEvent_t evMid; bool midValid;                 // "allocation + integration of the last frame are done" (pipelined uploads wait for it)         // B200_GRAPH=1: the fused frame is captured and replayed as a CUDA graph
   float *d_viewScratch; size_t viewScratchPixels;   // plays view->depth inside UpdateView (view.cu)
-  cudaEvent_t *evRing;                // timing mode 2: event pairs around every integrate launch
-  int evRingCap, evRingCount, timingMode;
+  unsigned long long *d_spans;        // timing modes 2 to 4: %globaltimer spans of the chain's kernels, per fused frame (span_slot)
+  int spanCount, timingMode;          // fused frames stamped since the mode was set
   // timing mode 3: an event pair around every kernel launch (launch trace, b200_get_trace)
   bool traceOn; int traceCount, traceCap; cudaEvent_t *traceEv; const char **traceName;
   // expected-depth cells outside the live corner of the latest fused frame: rasterised lazily at b200_sync()
@@ -134,13 +136,14 @@ void launch_push_snapshot(b200_engine *e, const b200_vec3i *positions, int n, in
 // launchers (each enqueues on e->stream and bumps e->launches)
 void launch_reset(b200_engine *e, const SceneRef &s);
 void launch_allocate(b200_engine *e, const SceneRef &s, const FrameGeom &g, const float *depth, bool onlyVisible,
-                     int frameIdx, int snapSlot, b200_vec2f *minmaxDead, int mw, int mh);
-void launch_integrate(b200_engine *e, const SceneRef &s, const FrameGeom &g, const float *depth, const b200_vec4u *rgb);
+                     int frameIdx, int snapSlot, b200_vec2f *minmaxDead, int mw, int mh, bool fused = false);
+// fused = true: a launch of the fused frame's chain (launch_chained), stamped in timing modes 2 and 4
+void launch_integrate(b200_engine *e, const SceneRef &s, const FrameGeom &g, const float *depth, const b200_vec4u *rgb, bool fused = false);
 void integrate_init_device(b200_engine *e);   // per-device: division table upload, dynamic shared-memory attributes
 static inline const int *fresh_ptr_list(const b200_engine *e, const SceneRef &s) {
   return (e->ptrListFor == (const void *)s.visiblePos && e->ptrListVersion == e->tableVersion) ? e->d_visiblePtr : nullptr;
 }
-void launch_decay_partial(b200_engine *e, const SceneRef &s, int snapSlot, int minAge, int maxWeight, int frameIdx);
+void launch_decay_partial(b200_engine *e, const SceneRef &s, int snapSlot, int minAge, int maxWeight, int frameIdx, bool fused = false);
 void launch_decay_full(b200_engine *e, const SceneRef &s, int minAge, int maxWeight, int frameIdx);
 // FindVisibleBlocks into s.visiblePos; the count, the tile ticket and the scan descriptors (FV_TILE entries per tile) are the
 // caller's, so that the free-view preview keeps its own
@@ -155,7 +158,7 @@ void launch_expected_depths(b200_engine *e, const SceneRef &s, const Mat4 &M, co
 // the fused frame's expected-depth cells outside the live corner, from the block records of its allocation
 void launch_expected_depths_dead(b200_engine *e, const SceneRef &s, int w, int h, b200_vec2f *minmax);
 void launch_raycast(b200_engine *e, const SceneRef &s, const Mat4 &invM, const float proj[4], int w, int h, float voxelSize,
-                    float mu, const b200_vec2f *minmax, b200_vec4f *out);
+                    float mu, const b200_vec2f *minmax, b200_vec4f *out, bool fused = false);
 void launch_shade(b200_engine *e, const SceneRef &s, const Mat4 &M, const Mat4 &invM, int w, int h, float voxelSize, int maxW,
                   const b200_vec4f *rays, b200_vec4u *outChar, float *outDepth, int type);
 void launch_icp(b200_engine *e, const Mat4 &invM, int w, int h, float voxelSize, const b200_vec4f *rays, b200_vec4u *outImg,
@@ -202,6 +205,38 @@ static inline void trace_end(b200_engine *e, cudaStream_t st) {
   e->traceCount++;
 }
 #define TRACED(e, st, name, ...) do { trace_begin(e, st, name); __VA_ARGS__; trace_end(e, st); } while (0)
+
+// Launch of a kernel of the fused frame's main-stream chain k_mark_prepare -> k_serve_list -> k_integrate_v4 -> k_raycast ->
+// k_decay_blocks<0>. With chained = true the launch carries programmatic stream serialisation: its CTAs may become resident and
+// run the code before their pdl_wait() while the previous kernel of the stream drains. Rules kept by every kernel of the chain:
+//  * a kernel calls pdl_trigger() only after its own pdl_wait() has returned. By induction, when a kernel runs its pre-wait code,
+//    everything two or more launches back has completed and its memory is visible;
+//  * pre-wait code reads only data whose last writer is at least two launches back, or that the caller wrote before the
+//    frame's first launch (k_mark_prepare, launched with chained = false, waits for everything enqueued before it);
+//  * pre-wait code writes only scratch that the previous kernel neither reads nor writes;
+//  * no stream operation (event record, copy, memset) sits between two chained launches: it would serialise them again.
+// Stand-alone entry points launch with chained = false; pdl_wait() is then a no-op and the kernels are unchanged.
+template <typename... KArgs, typename... Args>
+static inline void launch_chained(bool chained, void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t st,
+                                  Args &&...args) {
+  cudaLaunchAttribute attr[1];
+  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+  attr[0].val.programmaticStreamSerializationAllowed = 1;
+  cudaLaunchConfig_t cfg = {};
+  cfg.gridDim = grid; cfg.blockDim = block; cfg.dynamicSmemBytes = smem; cfg.stream = st;
+  cfg.attrs = attr; cfg.numAttrs = chained ? 1 : 0;
+  cudaLaunchKernelEx(&cfg, kernel, std::forward<Args>(args)...);
+}
+
+// %globaltimer spans of the chain's kernels (b200_set_timing modes 2 to 4): one record of SPAN_KERNELS SpanStamp slots per fused
+// frame, SPAN_FRAMES records, zero-filled whenever the mode is set. Mode 2 stamps the integrate kernel only.
+enum { SPAN_MARK, SPAN_SERVE, SPAN_INTEGRATE, SPAN_RAYCAST, SPAN_DECAY, SPAN_KERNELS };
+#define SPAN_FRAMES 8192
+// the slot of kernel k in the record of the fused frame being enqueued, or nullptr when that kernel is not stamped
+static inline unsigned long long *span_slot(const b200_engine *e, int k) {
+  if (e->timingMode < 2 || !e->d_spans || e->spanCount >= SPAN_FRAMES || (e->timingMode == 2 && k != SPAN_INTEGRATE)) return nullptr;
+  return e->d_spans + ((size_t)e->spanCount * SPAN_KERNELS + k) * 2;
+}
 
 #define DECAY_CAND_CAP 1024
 

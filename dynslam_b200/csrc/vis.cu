@@ -275,7 +275,7 @@ template <bool useNbr>
 __global__ void __launch_bounds__(RC_THREADS)
 k_raycast(float4 *out, const b200_voxel *__restrict__ voxels, const b200_hash_entry *__restrict__ table, int nb, int w, int h, Mat4 invM,
           float fx, float fy, float cxp, float cyp, float voxelSize, float mu, const float2 *__restrict__ minmax, int twLog2, int centreRow,
-          int tilesX, int tilesY, unsigned tilesXMagic) {
+          int tilesX, int tilesY, unsigned tilesXMagic, unsigned long long *span) {
   // warp tile: (1 << twLog2) x (32 >> twLog2) pixels
   const int tw = 1 << twLog2, th = 32 >> twLog2;
   const int warpGlobal = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
@@ -294,18 +294,24 @@ k_raycast(float4 *out, const b200_voxel *__restrict__ voxels, const b200_hash_en
   const int x = (warpGlobal - rowLinear * tilesX) * tw + (lane & (tw - 1)), y = tileRow * th + (lane >> twLog2);
   if (x >= w || y >= h) return;
   const int locId2 = (int)floorf((float)x / B200_MINMAX_SUBSAMPLE) + (int)floorf((float)y / B200_MINMAX_SUBSAMPLE) * w;
+  // In the fused frame the expected-depth image was last written by the list kernel, two launches back (launch_chained's rules):
+  // it is read before the wait for the integrate kernel, which writes only voxels.
+  const float2 mm = __ldg(minmax + locId2);
+  pdl_wait();
+  pdl_trigger();
+  SpanStamp stamp(span);
   float4 o;
   if (useNbr) {
     __shared__ int nbr[8][RC_THREADS];     // per thread: the 2x2x2 block neighbourhood of the ray's current block (raycast_ray.cuh)
-    cast_ray_nbr(o, x, y, voxels, table, nb, invM, 1.0f / fx, 1.0f / fy, cxp, cyp, 1.0f / voxelSize, mu, __ldg(minmax + locId2), &nbr[0][threadIdx.x], RC_THREADS);
+    cast_ray_nbr(o, x, y, voxels, table, nb, invM, 1.0f / fx, 1.0f / fy, cxp, cyp, 1.0f / voxelSize, mu, mm, &nbr[0][threadIdx.x], RC_THREADS);
   } else {
-    cast_ray(o, x, y, voxels, table, nb, invM, 1.0f / fx, 1.0f / fy, cxp, cyp, 1.0f / voxelSize, mu, __ldg(minmax + locId2));
+    cast_ray(o, x, y, voxels, table, nb, invM, 1.0f / fx, 1.0f / fy, cxp, cyp, 1.0f / voxelSize, mu, mm);
   }
   out[x + y * w] = o;
 }
 
 void launch_raycast(b200_engine *e, const SceneRef &s, const Mat4 &invM, const float proj[4], int w, int h, float voxelSize, float mu,
-                    const b200_vec2f *minmax, b200_vec4f *out) {
+                    const b200_vec2f *minmax, b200_vec4f *out, bool fused) {
   const int twLog2 = e->rcTileLog2;   // warp tile (1 << twLog2) x (32 >> twLog2) pixels; 3: 8x4 (default)
   const int tw = 1 << twLog2, th = 32 >> twLog2;
   const int tiles = ((w + tw - 1) / tw) * ((h + th - 1) / th);
@@ -321,14 +327,9 @@ void launch_raycast(b200_engine *e, const SceneRef &s, const Mat4 &invM, const f
   const unsigned magic = (unsigned)((0x100000000ull + (unsigned)tilesXh - 1) / (unsigned)tilesXh);
   const int impl = e->rcImpl;   // 1: neighbourhood cache (default); 0: per-lane one-entry cache (cross-check)
   trace_begin(e, e->stream, "k_raycast");
-  if (impl)
-    k_raycast<true><<<(tiles + warpsPerCta - 1) / warpsPerCta, RC_THREADS, 0, e->stream>>>((float4 *)out, s.voxels, s.hash, s.numBuckets, w, h, invM,
-                                                                                          proj[0], proj[1], proj[2], proj[3], voxelSize, mu,
-                                                                                          (const float2 *)minmax, twLog2, centreRow, tilesXh, tilesYh, magic);
-  else
-    k_raycast<false><<<(tiles + warpsPerCta - 1) / warpsPerCta, RC_THREADS, 0, e->stream>>>((float4 *)out, s.voxels, s.hash, s.numBuckets, w, h, invM,
-                                                                                           proj[0], proj[1], proj[2], proj[3], voxelSize, mu,
-                                                                                           (const float2 *)minmax, twLog2, centreRow, tilesXh, tilesYh, magic);
+  launch_chained(fused, impl ? k_raycast<true> : k_raycast<false>, (tiles + warpsPerCta - 1) / warpsPerCta, RC_THREADS, 0, e->stream,
+                 (float4 *)out, s.voxels, s.hash, s.numBuckets, w, h, invM, proj[0], proj[1], proj[2], proj[3], voxelSize, mu,
+                 (const float2 *)minmax, twLog2, centreRow, tilesXh, tilesYh, magic, fused ? span_slot(e, SPAN_RAYCAST) : nullptr);
   trace_end(e, e->stream);
   e->launches++;
 }

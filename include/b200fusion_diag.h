@@ -14,16 +14,19 @@ typedef struct {
   float ms_allocate, ms_integrate, ms_expected, ms_raycast, ms_decay, ms_total;
   int64_t launches;            /* kernels launched by this engine since creation */
   int32_t noVisibleBlocks, noIntegratedBlocks;
-  /* timing mode 2: CUDA-event pairs around EVERY IntegrateIntoScene launch since the mode was set */
+  /* timing modes 2 to 4: every IntegrateIntoScene launch of a fused frame since the mode was set, timed by the kernel's own
+     %globaltimer stamps (first CTA past its dependency wait to the last warp's exit; b200_diag_read_spans) */
   float ring_ms_integrate;     /* sum of the launch durations */
   int32_t ring_count;          /* number of launches measured */
   int64_t totalIntegratedBlocks; /* cumulative blocks integrated since engine creation */
   int64_t droppedSnapshots;    /* decay-queue snapshots dropped because the queue or the ring was full (b200_engine_config) */
 } b200_frame_stats;
 
-/* 0 = off; 1 = per-stage CUDA events of the last fused frame; 2 = 1 + an event pair around every
-   integrate launch (ring of 8192 frames), reset whenever the mode is set; 3 = an event pair around EVERY
-   kernel launch of the frame path (launch trace, read and cleared by b200_get_trace; perturbs the timing) */
+/* 0 = off; 1 = per-stage CUDA events of the last fused frame (between the chained kernels: they serialise the chain);
+   2 = the fused frame's time (events before and after it only) + %globaltimer spans of every integrate launch (8192 frames),
+   reset whenever the mode is set; 3 = 1 + an event pair around EVERY kernel launch of the frame path (launch trace, read and
+   cleared by b200_get_trace; perturbs the timing) + the spans of mode 4; 4 = 2 with the spans of all five kernels of the
+   fused frame's main-stream chain (b200_diag_read_spans), no events inside the chain */
 void b200_set_timing(b200_engine *e, int enabled);
 /* "kernel start_us end_us" lines (relative to the first traced launch); returns the number of bytes written */
 int b200_get_trace(b200_engine *e, char *out, int cap);
@@ -53,6 +56,13 @@ void b200_diag_last_integrate(const b200_engine *e, int *kernel, int *grid);
    measures block ages against). Tests use both to hand the engine exactly the decay state they hand the oracle. */
 b200_status b200_diag_push_decay_snapshot(b200_engine *e, const b200_vec3i *d_positions, int n);
 void b200_diag_set_frame_index(b200_engine *e, int32_t f);
+
+/* Kernel spans of the fused frames stamped since b200_set_timing(e, 2 | 3 | 4) (at most 8192 frames, at most maxFrames copied):
+   per frame 5 kernels (k_mark_prepare, k_serve_list, the integrate kernel, k_raycast, k_decay_blocks<0>) x {first CTA entry
+   after the kernel's dependency wait, last warp exit}, %globaltimer nanoseconds, 0 where the kernel did not run or was not
+   stamped (mode 2 stamps the integrate kernel only). Synchronises the engine's stream; returns the number of frames copied.
+   Measurement only. */
+int b200_diag_read_spans(b200_engine *e, unsigned long long *out, int maxFrames);
 
 /* While the launch trace is on (b200_set_timing(e, 3)) a few CTAs of the allocation's list pass stamp %globaltimer at their
    phase boundaries (8 stamps x 4 CTAs, nanoseconds); copies up to 64 of them out. Measurement only. */

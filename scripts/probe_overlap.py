@@ -1,0 +1,113 @@
+"""GPU probe: where the fused frame's main-stream chain spends its time between kernels, without events inside the chain.
+
+Runs the bench configuration (1242x375 KITTI-shaped stream, 0x60000 blocks, 0x100000 + 0x80000 entries, decay maxWeight 1 /
+minAge 200, 230-frame pre-roll so partial decay is live, L2 flushed before every frame) and reads the kernels' own %globaltimer
+stamps (b200_set_timing(4), b200_diag_read_spans): per kernel the first CTA's entry after its dependency wait and the last warp's
+exit. Prints, as medians over the measured frames, each kernel's span, the idle time at each of the four boundaries (next
+entry - previous exit) and the frame's chain from the first entry to the last exit.
+
+Then mode 3 (an event pair around every launch, which serialises the chain) for the same number of frames: the integrate
+kernel's stamp span against its event pair, launch by launch — the check that the stamps time the integrate launch as the
+events did — and the smallest step of %globaltimer seen in the stamps.
+
+    python scripts/probe_overlap.py [--frames 200] [--json out.json]
+"""
+import argparse, ctypes as C, json, os, sys
+sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+import numpy as np, torch
+from dynslam_b200 import engine as E, synth
+import bench
+
+NAMES = ["k_mark_prepare", "k_serve_list", "k_integrate", "k_raycast", "k_decay_blocks<0>"]
+
+
+def read_spans(eng, n):
+    buf = (C.c_uint64 * (n * len(NAMES) * 2))()
+    got = eng.lib.b200_diag_read_spans(eng.h, buf, n)
+    return np.frombuffer(buf, dtype=np.uint64, count=got * len(NAMES) * 2).reshape(got, len(NAMES), 2).astype(np.int64)
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--frames", type=int, default=200)
+    ap.add_argument("--preroll", type=int, default=230)
+    ap.add_argument("--json", default=None)
+    args = ap.parse_args()
+    dev = torch.device("cuda:0")
+    W, H = synth.KITTI_W, synth.KITTI_H
+    n = args.frames
+    total = args.preroll + 2 * n + 4
+    frames = bench.gen_frames_parallel(6, 0, total, total * 0.8 + 60.0, max(1, min(16, os.cpu_count() or 2)))
+    scene = E.Scene(E.SceneParams(), bench.NUM_BLOCKS, bench.NUM_BUCKETS, bench.EXCESS, device="cuda:0")
+    eng = E.Engine(scene, (W, H))
+    reco = E.SceneReconstructionEngine(eng)
+    rs = E.VisualisationEngine(eng, scene).CreateRenderState((W, H))
+    reco.ResetScene(scene)
+    points = torch.zeros((H, W, 4), dtype=torch.float32, device=dev)
+    normals = torch.zeros((H, W, 4), dtype=torch.float32, device=dev)
+    flush = torch.zeros(256 * 1024 * 1024 // 4, dtype=torch.int32, device=dev)
+    view = lambda f: E.View(torch.from_numpy(f[0]).to(dev), torch.from_numpy(f[1]).to(dev), f[2], f[3])
+    idx = 0
+    for _ in range(args.preroll):
+        eng.process_frame_async(rs, view(frames[idx]), points, normals, decay=bench.DECAY); idx += 1
+    eng.sync(rs)
+    props = torch.cuda.get_device_properties(dev)
+    out = {"device": props.name}
+
+    # ---- mode 4: stamps only, the chain as the benchmark runs it ----
+    views = [view(frames[idx + i]) for i in range(n)]; idx += n
+    torch.cuda.synchronize()
+    eng.set_timing(4)
+    for v in views:
+        flush.add_(1)
+        eng.process_frame_async(rs, v, points, normals, decay=bench.DECAY)
+    eng.sync(rs)
+    sp = read_spans(eng, n)
+    eng.set_timing(0)
+    ok = (sp[:, :, 0] > 0).all(axis=1) & (sp[:, :, 1] > 0).all(axis=1)
+    sp = sp[ok]
+    us = lambda a: float(np.median(a)) / 1000.0
+    spans = {NAMES[k]: us(sp[:, k, 1] - sp[:, k, 0]) for k in range(len(NAMES))}
+    gaps = {f"{NAMES[k]} -> {NAMES[k + 1]}": us(sp[:, k + 1, 0] - sp[:, k, 1]) for k in range(len(NAMES) - 1)}
+    chain = us(sp[:, -1, 1] - sp[:, 0, 0])
+    out.update({"frames": int(ok.sum()), "span_us": spans, "idle_us": gaps, "chain_us": chain,
+                "sum_of_spans_us": sum(spans.values()), "sum_of_idle_us": sum(gaps.values())})
+    print(f"device {props.name}; {int(ok.sum())} frames with every kernel stamped (medians, us)")
+    for k, v in spans.items():
+        print(f"  span  {k:<20s} {v:7.2f}")
+    for k, v in gaps.items():
+        print(f"  idle  {k:<40s} {v:7.2f}   (negative: the next kernel's first CTA passed its wait before the last warp left)")
+    print(f"  chain first entry -> last exit {chain:7.2f}; spans {sum(spans.values()):.2f} + idle {sum(gaps.values()):.2f}")
+
+    # ---- mode 3: the integrate kernel's stamps against an event pair around each launch (no overlap: events in the chain) ----
+    views = [view(frames[idx + i]) for i in range(n)]; idx += n
+    torch.cuda.synchronize()
+    eng.set_timing(3)
+    ev_us = []
+    for v in views:
+        flush.add_(1)
+        eng.process_frame_async(rs, v, points, normals, decay=bench.DECAY)
+        eng.sync(rs)
+        ev_us += [b - a for name, a, b in eng.trace() if name.startswith("k_integrate")]
+    sp3 = read_spans(eng, n)
+    eng.set_timing(0)
+    st_us = (sp3[:, 2, 1] - sp3[:, 2, 0]) / 1000.0
+    m = min(len(ev_us), len(st_us))
+    d = np.asarray(st_us[:m]) - np.asarray(ev_us[:m])
+    stamps = np.unique(np.concatenate([sp[:, :, 0].ravel(), sp[:, :, 1].ravel()]))
+    steps = np.diff(stamps)
+    res = int(steps[steps > 0].min()) if (steps > 0).any() else 0
+    out.update({"integrate_events_us": float(np.median(ev_us[:m])), "integrate_stamps_us": float(np.median(st_us[:m])),
+                "stamp_minus_event_us": {"median": float(np.median(d)), "p10": float(np.percentile(d, 10)), "p90": float(np.percentile(d, 90))},
+                "globaltimer_step_ns": res})
+    print(f"integrate, mode 3, {m} launches: event pair {np.median(ev_us[:m]):.2f} us, stamps {np.median(st_us[:m]):.2f} us; "
+          f"stamps - events: median {np.median(d):.2f}, p10 {np.percentile(d, 10):.2f}, p90 {np.percentile(d, 90):.2f} us")
+    print(f"smallest %globaltimer step between distinct stamps: {res} ns")
+    if args.json:
+        os.makedirs(os.path.dirname(os.path.abspath(args.json)), exist_ok=True)
+        with open(args.json, "w") as f:
+            json.dump(out, f, indent=1)
+
+
+if __name__ == "__main__":
+    main()
