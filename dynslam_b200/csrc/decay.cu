@@ -8,16 +8,15 @@
 // The reference takes a per-bucket lock (4 MiB array memset per call), DROPS a deletion when the
 // lock is contended, and pushes freed slots with atomicAdd — nondeterministic. Here the pass is
 // split so that it equals the serial oracle (blocks in list order):
-//   phase 1  per list item, one CTA iteration: resolve the block once, sweep its 4 KiB with 128-bit
-//            loads, reset noisy voxels, decide "block is empty" with a block-wide vote; the first
-//            item (list order) that empties a block claims it with a 64-bit atomicMax tag;
+//   phase 1  the sweep (decay_sweep.cuh), one warp per list item: resolve the block once, read its 4 KiB with 128-bit loads,
+//            apply the reset rule, decide "block is empty" with a warp-wide vote; the first item (list order) that empties a
+//            block claims it with a 64-bit atomicMax tag. A full decay stores the resets as it goes; a partial one only
+//            records which blocks have voxels to reset, and k_decay_commit stores them;
 //   phase 2  ordered compaction of the claiming items => free-list position = rank in list order;
 //   phase 3  chain leaders: for every bucket chain that loses blocks, ONE thread applies that
 //            chain's deletions in list order with the reference's unlink rules (incl. the
 //            visibility-byte moves and the never-reclaimed excess slots, :1075-1111).
-#include "engine.h"
-
-DEV unsigned long long del_tag(unsigned gen, unsigned item) { return ((unsigned long long)gen << 32) | (0xffffffffu - item); }
+#include "decay_sweep.cuh"
 
 DEV void item_pos(int mode, const b200_vec3i *ring, long long ringCap, long long s0, const short4 *allocatedPos, int item, int &x, int &y, int &z);
 DEV bool chain_leader(const b200_hash_entry *table, int numBuckets, int x, int y, int z, int item, const unsigned long long *delTag, unsigned gen);
@@ -26,93 +25,50 @@ __device__ void decay_commit_body(b200_hash_entry *table, int numBuckets, uint8_
                                   const int *itemPtr, const unsigned long long *delTag, unsigned gen, int *allocList, int *delList,
                                   uint8_t *isLeader, DevCounters *ctr, const int *candList, unsigned *sm, int *cand);
 
-// phase 1. MODE 0: items = ring snapshot; MODE 1: items = VBA slots with allocatedPos.w != 0
+// phase 1 as a grid of its own: full decay (MODE 1), and a partial one (MODE 0) when no raycast carries its sweep
 template <int MODE>
+__global__ void __launch_bounds__(256) k_decay_sweep(DecaySweep d) {
+  pdl_wait();            // in a fused frame without a raycast: the integrate kernel writes the voxels this sweep reads
+  pdl_trigger();
+  SpanStamp stamp(d.span);
+  decay_sweep<MODE>(d, (blockIdx.x * blockDim.x + threadIdx.x) >> 5, gridDim.x * (blockDim.x >> 5));
+}
+
+// Partial decay, after everything that reads the voxels: the reset stores of the sweep, then phases 2 + 3 + counters. A warp
+// per item the sweep flagged reloads its block and applies the reset rule again: nothing has written those voxels since the
+// sweep read them, so the rule changes the same voxels to the same bits. The CTA that finishes last commits the pass.
 __global__ void __launch_bounds__(256)
-k_decay_blocks(b200_voxel *voxels, const b200_hash_entry *table, int numBuckets, const b200_vec3i *ring,
-               long long ringCap, const long long *snapStart, const int *snapCount, int slot, const short4 *allocatedPos,
-               int numBlocks, int minAge, int maxWeight, int currentFrame, unsigned gen, unsigned long long *delTag,
-               int *itemPtr, DevCounters *ctr, int *candList, uint8_t *visType, int *allocList, int *delList, uint8_t *isLeader,
+k_decay_commit(b200_voxel *voxels, int maxWeight, const int *resetPtr, b200_hash_entry *table, int numBuckets, const b200_vec3i *ring,
+               long long ringCap, const long long *snapStart, int slot, unsigned gen, const unsigned long long *delTag, const int *itemPtr,
+               DevCounters *ctr, const int *candList, uint8_t *visType, int *allocList, int *delList, uint8_t *isLeader,
                unsigned long long *span) {
-  pdl_wait();            // in the fused frame: the raycast reads the voxels and entries this sweep resets and unlinks
+  pdl_wait();            // in the fused frame: the raycast reads the voxels and entries this kernel resets and unlinks
   SpanStamp stamp(span);
-  // One WARP per list item (a block = 256 uint4 = 8 per lane, all 8 loads in flight), 8 items per CTA: the per-item chain of
-  // dependent loads (ring position -> hash chain -> voxels) overlaps across warps, so the few thousand items of a frame are
-  // one wave of warps instead of ~5 sequential items per CTA.
   const int lane = threadIdx.x & 31;
-  const int warpsTotal = gridDim.x * (blockDim.x >> 5), warpId = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
-  int n = (MODE == 0) ? snapCount[slot] : numBlocks;
-  const long long s0 = (MODE == 0) ? snapStart[slot] : 0;
-  // a snapshot the ring has wrapped over since it was taken is gone (b200_engine_config.decayRingItems): sweep nothing
-  const bool overwritten = (MODE == 0) && (ctr->ringHead - s0 > ringCap);
-  if (overwritten) n = 0;
-  if (blockIdx.x == 0 && threadIdx.x == 0) { ctr->decayItems = n; if (overwritten) ctr->droppedSnapshots++; }
-  for (int item = warpId; item < n; item += warpsTotal) {
-    int x, y, z;
-    if (MODE == 0) { b200_vec3i p = ring[(s0 + item) % ringCap]; x = p.x; y = p.y; z = p.z; }
-    else {
-      short4 p = allocatedPos[item];
-      if (p.w == 0) { if (lane == 0) itemPtr[item] = -1; continue; }
-      x = p.x; y = p.y; z = p.z;
-    }
-    // findBlock / findVoxel (:1214, :1138): uniform across the warp
-    int idx = hash_index(x, y, z, numBuckets - 1), ptr = -1, allocatedTime = 0;
-    for (;;) {
-      const int *w = reinterpret_cast<const int *>(table) + (size_t)idx * 5;
-      int w0 = w[0], w1 = w[1], off = w[2], p = w[3];     // plain loads: the last CTA of a partial sweep rewrites the table (commit)
-      if ((short)(w0 & 0xffff) == x && (short)(w0 >> 16) == y && (short)(w1 & 0xffff) == z && p >= 0) {
-        ptr = p; allocatedTime = w[4]; break;
-      }
-      if (off < 1) break;
-      idx = numBuckets + off - 1;
-    }
-    bool claim = false;
-    if (ptr >= 0 && (currentFrame - allocatedTime) >= minAge) {   // safeToClear (:1151-1157)
-      uint4 *blk = reinterpret_cast<uint4 *>(voxels + (size_t)ptr * BS3) + lane;
-      uint4 raw[8];
+  const int warps = gridDim.x * (blockDim.x >> 5), warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+  const int n = ctr->decayItems;
+  for (int item = warp; item < n; item += warps) {
+    const int ptr = resetPtr[item];
+    if (ptr < 0) continue;
+    uint4 *blk = reinterpret_cast<uint4 *>(voxels + (size_t)ptr * BS3) + lane;
+    uint4 raw[8];
 #pragma unroll
-      for (int k = 0; k < 8; ++k) raw[k] = ld_stream(blk + 32 * k);
-      int empty = 0;
+    for (int k = 0; k < 8; ++k) raw[k] = ld_stream(blk + 32 * k);
+    int empty = 0;
 #pragma unroll
-      for (int k = 0; k < 8; ++k) {
-        bool ch = false;
-        int wd = (raw[k].x >> 16) & 0xff;
-        if (wd <= maxWeight && wd > 0) { raw[k].x = 0x00007fffu; raw[k].y &= 0xff000000u; ch = true; wd = 0; }
-        empty += (wd == 0);
-        wd = (raw[k].z >> 16) & 0xff;
-        if (wd <= maxWeight && wd > 0) { raw[k].z = 0x00007fffu; raw[k].w &= 0xff000000u; ch = true; wd = 0; }
-        empty += (wd == 0);
-        if (ch) st_stream(blk + 32 * k, raw[k]);
-      }
-      // block-wide count of empty voxels (replaces the 512-int shared-memory tree, ITMCUDAUtils.h:145-160)
-      for (int o = 16; o > 0; o >>= 1) empty += __shfl_xor_sync(0xffffffffu, empty, o);
-      claim = (empty == BS3);
-    }
-    if (lane == 0) {
-      itemPtr[item] = claim ? ptr : -1;
-      if (claim) {
-        atomicMax(&delTag[ptr], del_tag(gen, (unsigned)item));
-        if (MODE == 0) {   // remember the candidate: the commit ranks the few of them instead of scanning the whole list
-          const int c = atomicAdd(&ctr->decayCand, 1);
-          if (c < DECAY_CAND_CAP) candList[c] = item;
-        }
-      }
-    }
+    for (int k = 0; k < 8; ++k) if (decay_reset_pair(raw[k], maxWeight, empty)) st_stream(blk + 32 * k, raw[k]);
   }
-  if (MODE == 0) {
-    // partial decay: the CTA that finishes last commits the pass (rank, elect, unlink, counters) — no second launch
-    __shared__ bool lastCta;
-    __shared__ unsigned smScan[33];
-    __shared__ int smCand[DECAY_CAND_CAP];
-    __threadfence();
-    __syncthreads();
-    if (threadIdx.x == 0) lastCta = (atomicAdd(&ctr->decayCtasDone, 1u) == gridDim.x - 1);
-    __syncthreads();
-    if (!lastCta) return;
-    __threadfence();
-    decay_commit_body(const_cast<b200_hash_entry *>(table), numBuckets, visType, ring, ringCap, s0, itemPtr, delTag, gen, allocList, delList,
-                      isLeader, ctr, candList, smScan, smCand);
-  }
+  __shared__ bool lastCta;
+  __shared__ unsigned smScan[33];
+  __shared__ int smCand[DECAY_CAND_CAP];
+  __threadfence();
+  __syncthreads();
+  if (threadIdx.x == 0) lastCta = (atomicAdd(&ctr->decayCtasDone, 1u) == gridDim.x - 1);
+  __syncthreads();
+  if (!lastCta) return;
+  __threadfence();
+  decay_commit_body(table, numBuckets, visType, ring, ringCap, snapStart[slot], itemPtr, delTag, gen, allocList, delList, isLeader, ctr,
+                    candList, smScan, smCand);
 }
 
 // phase 2: ordered compaction of the claiming items, free-list push by rank (:1072-1073)
@@ -253,9 +209,9 @@ __global__ void k_decay_unlink(b200_hash_entry *table, int numBuckets, uint8_t *
   }
 }
 
-// phases 2 + 3 + counters of a PARTIAL decay, run by the LAST CTA of the sweep (k_decay_blocks<0>) — a frame's list is a few
-// thousand items and the few dozen blocks it empties are known as unordered candidates by then; a second launch for this cost
-// 13 us of the frame. Ordered compaction of the claims, leader election, chain unlinking, counter update. All threads of the
+// phases 2 + 3 + counters of a PARTIAL decay, run by the LAST CTA of k_decay_commit — a frame's list is a few thousand items
+// and the few dozen blocks it empties are known as unordered candidates by then; a launch of its own for this cost 13 us of
+// the frame. Ordered compaction of the claims, leader election, chain unlinking, counter update. All threads of the
 // calling CTA take part; reads of what other CTAs produced go to L2 (__ldcg).
 __device__ void decay_commit_body(b200_hash_entry *table, int numBuckets, uint8_t *visType, const b200_vec3i *ring, long long ringCap, long long s0,
                                   const int *itemPtr, const unsigned long long *delTag, unsigned gen, int *allocList, int *delList,
@@ -363,46 +319,53 @@ void launch_push_snapshot(b200_engine *e, const b200_vec3i *positions, int n, in
   e->launches++;
 }
 
-static void decay_common(b200_engine *e, const SceneRef &s, int mode, int slot, int minAge, int maxWeight, int frameIdx,
-                         long long items, bool fused = false) {
-  cudaStream_t st = e->stream;
-  const unsigned gen = ++e->decayGen;
-  const int grid1 = persistent_grid(e, 6, (items + 7) / 8);   // 8 items (warps) per CTA
-  if (mode == 0) {
-    trace_begin(e, st, "k_decay_blocks<0>");
-    launch_chained(fused, k_decay_blocks<0>, grid1, 256, 0, st, s.voxels, s.hash, s.numBuckets, e->d_ring, e->ringCap, e->d_snapStart,
-                   e->d_snapCount, slot, e->d_allocatedPos, s.numBlocks, minAge, maxWeight, frameIdx, gen, e->d_delTag, e->d_itemPtr,
-                   e->d_ctr, e->d_candList, s.visType, s.allocationList, e->d_delList, e->d_isLeader,
-                   fused ? span_slot(e, SPAN_DECAY) : nullptr);
-    trace_end(e, st);
-  } else {
-    trace_begin(e, st, "k_decay_blocks<1>");
-    k_decay_blocks<1><<<grid1, 256, 0, st>>>(s.voxels, s.hash, s.numBuckets, e->d_ring, e->ringCap, e->d_snapStart, e->d_snapCount,
-                                            slot, e->d_allocatedPos, s.numBlocks, minAge, maxWeight, frameIdx, gen, e->d_delTag,
-                                            e->d_itemPtr, e->d_ctr, e->d_candList, s.visType, s.allocationList, e->d_delList, e->d_isLeader,
-                                            nullptr);
-    trace_end(e, st);
-  }
-  if (mode == 0) { e->launches += 1; return; }   // the sweep's last CTA has committed the pass
-  const int noTiles = (int)((items + DEC_TILE - 1) / DEC_TILE);
-  k_decay_rank<<<persistent_grid(e, 4, noTiles), 256, 0, st>>>(e->d_itemPtr, e->d_delTag, gen, s.allocationList, e->d_delList,
-                                                               e->d_ctr, e->d_scanDesc, ++e->scanGen);
-  k_decay_elect<1><<<e->smCount, 128, 0, st>>>(s.hash, s.numBuckets, e->d_ring, e->ringCap, e->d_snapStart, slot, e->d_allocatedPos,
-                                              e->d_delList, e->d_delTag, gen, e->d_isLeader, e->d_ctr);
-  k_decay_unlink<<<e->smCount, 128, 0, st>>>(s.hash, s.numBuckets, s.visType, e->d_ring, e->ringCap, e->d_snapStart, slot,
-                                            e->d_allocatedPos, mode, e->d_delList, e->d_delTag, gen, e->d_isLeader, e->d_ctr);
-  k_decay_finish<<<1, 1, 0, st>>>(e->d_ctr);
-  e->launches += 5;
+DecaySweep decay_sweep_args(b200_engine *e, const SceneRef &s, int snapSlot, int minAge, int maxWeight, int frameIdx, bool fused) {
+  DecaySweep d;
+  d.voxels = s.voxels; d.table = s.hash; d.numBuckets = s.numBuckets; d.numBlocks = s.numBlocks;
+  d.ring = e->d_ring; d.ringCap = e->ringCap; d.snapStart = e->d_snapStart; d.snapCount = e->d_snapCount; d.slot = snapSlot;
+  d.allocatedPos = e->d_allocatedPos;
+  d.minAge = minAge; d.maxWeight = maxWeight; d.currentFrame = frameIdx; d.gen = ++e->decayGen;
+  d.delTag = e->d_delTag; d.itemPtr = e->d_itemPtr; d.resetPtr = e->d_resetPtr; d.candList = e->d_candList; d.ctr = e->d_ctr;
+  d.span = fused ? span_slot(e, SPAN_SWEEP) : nullptr;
+  return d;
 }
 
-void launch_decay_partial(b200_engine *e, const SceneRef &s, int snapSlot, int minAge, int maxWeight, int frameIdx, bool fused) {
-  // item count lives on the device (snapCount[slot]); size the grid for the capacity
-  decay_common(e, s, 0, snapSlot, minAge, maxWeight, frameIdx, s.numBlocks, fused);
+// 8 items (warps) per CTA; the item count lives on the device (snapCount[slot]), so the grid is sized for the capacity
+static int sweep_grid(const b200_engine *e, const SceneRef &s) { return persistent_grid(e, 6, ((long long)s.numBlocks + 7) / 8); }
+
+void launch_decay_partial(b200_engine *e, const SceneRef &s, const DecaySweep &d, bool swept, bool fused) {
+  cudaStream_t st = e->stream;
+  if (!swept) {
+    trace_begin(e, st, "k_decay_sweep<0>");
+    launch_chained(fused, k_decay_sweep<0>, sweep_grid(e, s), 256, 0, st, d);
+    trace_end(e, st);
+    e->launches++;
+  }
+  trace_begin(e, st, "k_decay_commit");
+  launch_chained(fused, k_decay_commit, persistent_grid(e, 2, ((long long)s.numBlocks + 7) / 8), 256, 0, st, s.voxels, d.maxWeight,
+                 (const int *)e->d_resetPtr, s.hash, s.numBuckets, (const b200_vec3i *)e->d_ring, e->ringCap, (const long long *)e->d_snapStart,
+                 d.slot, d.gen, (const unsigned long long *)e->d_delTag, (const int *)e->d_itemPtr, e->d_ctr, (const int *)e->d_candList,
+                 s.visType, s.allocationList, e->d_delList, e->d_isLeader, fused ? span_slot(e, SPAN_DECAY) : nullptr);
+  trace_end(e, st);
+  e->launches++;
 }
 
 void launch_decay_full(b200_engine *e, const SceneRef &s, int minAge, int maxWeight, int frameIdx) {
-  cudaMemsetAsync(e->d_allocatedPos, 0, sizeof(short4) * (size_t)s.numBlocks, e->stream);
-  k_find_allocated<<<e->smCount * 8, 256, 0, e->stream>>>(s.hash, s.noTotal, e->d_allocatedPos);
-  e->launches++;
-  decay_common(e, s, 1, 0, minAge, maxWeight, frameIdx, s.numBlocks);
+  cudaStream_t st = e->stream;
+  cudaMemsetAsync(e->d_allocatedPos, 0, sizeof(short4) * (size_t)s.numBlocks, st);
+  k_find_allocated<<<e->smCount * 8, 256, 0, st>>>(s.hash, s.noTotal, e->d_allocatedPos);
+  const DecaySweep d = decay_sweep_args(e, s, 0, minAge, maxWeight, frameIdx);
+  const unsigned gen = d.gen;
+  trace_begin(e, st, "k_decay_sweep<1>");
+  k_decay_sweep<1><<<sweep_grid(e, s), 256, 0, st>>>(d);
+  trace_end(e, st);
+  const int noTiles = (s.numBlocks + DEC_TILE - 1) / DEC_TILE;
+  k_decay_rank<<<persistent_grid(e, 4, noTiles), 256, 0, st>>>(e->d_itemPtr, e->d_delTag, gen, s.allocationList, e->d_delList,
+                                                               e->d_ctr, e->d_scanDesc, ++e->scanGen);
+  k_decay_elect<1><<<e->smCount, 128, 0, st>>>(s.hash, s.numBuckets, e->d_ring, e->ringCap, e->d_snapStart, 0, e->d_allocatedPos,
+                                              e->d_delList, e->d_delTag, gen, e->d_isLeader, e->d_ctr);
+  k_decay_unlink<<<e->smCount, 128, 0, st>>>(s.hash, s.numBuckets, s.visType, e->d_ring, e->ringCap, e->d_snapStart, 0,
+                                            e->d_allocatedPos, 1, e->d_delList, e->d_delTag, gen, e->d_isLeader, e->d_ctr);
+  k_decay_finish<<<1, 1, 0, st>>>(e->d_ctr);
+  e->launches += 6;
 }

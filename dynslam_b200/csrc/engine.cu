@@ -167,6 +167,7 @@ static b200_status engine_create_body(const b200_engine_config *cfg, b200_engine
   CK(cudaMemset(e->d_delTag, 0, sizeof(unsigned long long) * (size_t)e->numBlocks));
   CK(cudaMalloc(&e->d_visiblePtr, sizeof(int) * (size_t)e->numBlocks));
   CK(cudaMalloc(&e->d_itemPtr, sizeof(int) * (size_t)e->numBlocks));
+  CK(cudaMalloc(&e->d_resetPtr, sizeof(int) * (size_t)e->numBlocks));
   CK(cudaMalloc(&e->d_delList, sizeof(int) * (size_t)e->numBlocks));
   CK(cudaMalloc(&e->d_candList, sizeof(int) * DECAY_CAND_CAP));
   CK(cudaMalloc(&e->d_isLeader, (size_t)e->numBlocks));
@@ -212,7 +213,7 @@ void b200_engine_destroy(b200_engine *e) {
   cudaSetDevice(e->device);
   if (e->stream) cudaStreamSynchronize(e->stream);
   cudaFree(e->d_ctr); cudaFreeHost(e->h_ctr); cudaFree(e->d_reqKey); cudaFree(e->d_reqBits); cudaFree(e->d_markBytes); cudaFree(e->d_dbg); cudaFree(e->d_meshDesc); cudaFree(e->d_evalCounters); cudaFreeHost(e->h_evalCounters); cudaFree(e->d_scanDesc);
-  cudaFree(e->d_ring); cudaFree(e->d_snapCount); cudaFree(e->d_snapStart); cudaFree(e->d_delTag); cudaFree(e->d_itemPtr); cudaFree(e->d_visiblePtr);
+  cudaFree(e->d_ring); cudaFree(e->d_snapCount); cudaFree(e->d_snapStart); cudaFree(e->d_delTag); cudaFree(e->d_itemPtr); cudaFree(e->d_resetPtr); cudaFree(e->d_visiblePtr);
   cudaFree(e->d_viewScratch); cudaFree(e->d_delList); cudaFree(e->d_candList); cudaFree(e->d_isLeader); cudaFree(e->d_allocatedPos); cudaFree(e->d_tileCounts); cudaFree(e->d_blockRecs);
   for (int i = 0; i < 8; ++i) if (e->ev[i]) cudaEventDestroy(e->ev[i]);
   if (e->copyStream) {
@@ -379,16 +380,22 @@ b200_status b200_integrate(b200_engine *e, b200_scene *s, b200_render_state *rs,
   return download_sync(e, s, rs);
 }
 
-static void enqueue_decay(b200_engine *e, b200_scene *s, b200_render_state *rs, int maxWeight, int minAge, int forceAll,
-                          bool fused = false) {
-  SceneRef r = scene_ref(s, rs);
+// Host half of a partial Decay: when the oldest snapshot is minAge frames old, takes it off the queue and fills *d with its
+// sweep's arguments. Nothing is enqueued.
+static bool decay_due(b200_engine *e, const SceneRef &r, int maxWeight, int minAge, bool fused, DecaySweep *d) {
   e->tableVersion++;
-  if (forceAll) launch_decay_full(e, r, minAge, maxWeight, e->frameIdx);
-  else if ((long)e->qSize > minAge) {
-    const int slot = e->qHead % SNAP_SLOTS;
-    e->qHead++; e->qSize--;
-    launch_decay_partial(e, r, slot, minAge, maxWeight, e->frameIdx, fused);
-  }
+  if ((long)e->qSize <= minAge) return false;
+  const int slot = e->qHead % SNAP_SLOTS;
+  e->qHead++; e->qSize--;
+  *d = decay_sweep_args(e, r, slot, minAge, maxWeight, e->frameIdx, fused);
+  return true;
+}
+
+static void enqueue_decay(b200_engine *e, b200_scene *s, b200_render_state *rs, int maxWeight, int minAge, int forceAll) {
+  SceneRef r = scene_ref(s, rs);
+  DecaySweep d;
+  if (forceAll) { e->tableVersion++; launch_decay_full(e, r, minAge, maxWeight, e->frameIdx); }
+  else if (decay_due(e, r, maxWeight, minAge, false, &d)) launch_decay_partial(e, r, d, false);
 }
 
 b200_status b200_decay(b200_engine *e, b200_scene *s, b200_render_state *rs, int maxWeight, int minAge, int forceAll) {
@@ -638,14 +645,19 @@ static b200_status frame_enqueue(b200_engine *e, b200_scene *s, b200_render_stat
   // instead, the upload lands under the next frame's allocation pair and the pipelined frame rate drops by about 15 % on the H100.
   if (e->evMid && !e->useGraph) { CK(cudaEventRecord(e->evMid, e->stream)); e->midValid = true; }
   if (stages) CK(cudaEventRecord(e->ev[2], e->stream));
+  // Decay's queue bookkeeping comes before the raycast: a due partial pass runs its sweep on CTAs of the raycast's grid, and
+  // only its reset stores and its commit (k_decay_commit) wait for everything that reads the voxels.
+  DecaySweep dec;
+  const bool decay = opts && opts->doDecay && decay_due(e, r, opts->decayMaxWeight, opts->decayMinAge, true, &dec);
   if (doRay) {
     if (stages) CK(cudaEventRecord(e->ev[3], e->stream));
-    launch_raycast(e, r, g.invM_d, g.proj_d, rs->img_w, rs->img_h, s->voxelSize, s->mu, rs->d_minmax, rs->d_raycastResult, true);
+    launch_raycast(e, r, g.invM_d, g.proj_d, rs->img_w, rs->img_h, s->voxelSize, s->mu, rs->d_minmax, rs->d_raycastResult, true,
+                   decay ? &dec : nullptr);
     // optional colour render for compositing: reads voxel colours, so it has to run before this frame's decay resets any
     if (opts && opts->d_colourRender)
       launch_shade(e, r, g.M_d, g.invM_d, rs->img_w, rs->img_h, s->voxelSize, s->maxW, rs->d_raycastResult, opts->d_colourRender, nullptr,
                    B200_RENDER_COLOUR_FROM_VOLUME);
-    if (overlap) {   // the ICP-map pass (image space) runs beside the decay sweep (voxel space)
+    if (overlap) {   // the ICP-map pass (image space) runs beside the decay commit (voxel space)
       CK(cudaEventRecord(e->evFork, mainStream));
       CK(cudaStreamWaitEvent(e->sideStream, e->evFork, 0));
       e->stream = e->sideStream;
@@ -663,7 +675,7 @@ static b200_status frame_enqueue(b200_engine *e, b200_scene *s, b200_render_stat
     }
   } else if (stages) CK(cudaEventRecord(e->ev[3], e->stream));
   if (stages) CK(cudaEventRecord(e->ev[4], e->stream));
-  if (opts && opts->doDecay) enqueue_decay(e, s, rs, opts->decayMaxWeight, opts->decayMinAge, 0, true);
+  if (decay) launch_decay_partial(e, r, dec, doRay, true);
   if (overlap) CK(cudaStreamWaitEvent(mainStream, e->evJoin, 0));   // join: the frame is complete on the main stream
   if (e->timing) CK(cudaEventRecord(e->ev[5], e->stream));
   if (e->timingMode >= 2 && e->d_spans && e->spanCount < SPAN_FRAMES) e->spanCount++;

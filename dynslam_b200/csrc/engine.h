@@ -58,7 +58,7 @@ struct b200_engine {
   const void *ptrListFor;             // the visible list buffer d_visiblePtr describes
   unsigned long long tableVersion, ptrListVersion;   // d_visiblePtr is valid while they are equal
   int *d_itemPtr;                     // per decay item: VBA ptr (or -1)
-  unsigned *d_itemFlag;               // per decay item: 1 = deletes its block
+  int *d_resetPtr;                    // per partial-decay item: VBA ptr of its block when the sweep found voxels to reset (or -1)
   int *d_delList;                     // compacted deleting items (list order)
   int *d_candList;                    // DECAY_CAND_CAP unordered candidates of the partial pass (decay.cu)
   uint8_t *d_isLeader;
@@ -143,7 +143,29 @@ void integrate_init_device(b200_engine *e);   // per-device: division table uplo
 static inline const int *fresh_ptr_list(const b200_engine *e, const SceneRef &s) {
   return (e->ptrListFor == (const void *)s.visiblePos && e->ptrListVersion == e->tableVersion) ? e->d_visiblePtr : nullptr;
 }
-void launch_decay_partial(b200_engine *e, const SceneRef &s, int snapSlot, int minAge, int maxWeight, int frameIdx, bool fused = false);
+// Arguments of a decay sweep (decay_sweep.cuh). Partial decay: items = ring snapshot `slot`; full decay: VBA slots.
+struct DecaySweep {
+  b200_voxel *voxels;
+  const b200_hash_entry *table;
+  int numBuckets, numBlocks;
+  const b200_vec3i *ring;
+  long long ringCap;
+  const long long *snapStart;
+  const int *snapCount;
+  int slot;
+  const short4 *allocatedPos;
+  int minAge, maxWeight, currentFrame;
+  unsigned gen;
+  unsigned long long *delTag;
+  int *itemPtr, *resetPtr, *candList;
+  DevCounters *ctr;
+  unsigned long long *span;           // SpanStamp of the sweep (fused frame, timing modes 3 and 4), or nullptr
+};
+// A partial Decay of snapshot `snapSlot`, in two parts: the sweep (read and decide) and k_decay_commit (the reset stores and the
+// commit). decay_sweep_args takes the pass's generation; launch_decay_partial launches the sweep as a grid of its own unless
+// it already rode in the raycast's grid (swept = true: launch_raycast with the same arguments), then k_decay_commit.
+DecaySweep decay_sweep_args(b200_engine *e, const SceneRef &s, int snapSlot, int minAge, int maxWeight, int frameIdx, bool fused = false);
+void launch_decay_partial(b200_engine *e, const SceneRef &s, const DecaySweep &d, bool swept, bool fused = false);
 void launch_decay_full(b200_engine *e, const SceneRef &s, int minAge, int maxWeight, int frameIdx);
 // FindVisibleBlocks into s.visiblePos; the count, the tile ticket and the scan descriptors (FV_TILE entries per tile) are the
 // caller's, so that the free-view preview keeps its own
@@ -157,8 +179,9 @@ void launch_expected_depths(b200_engine *e, const SceneRef &s, const Mat4 &M, co
                             b200_vec2f *minmax, const int *count, unsigned *tiles, unsigned *done);
 // the fused frame's expected-depth cells outside the live corner, from the block records of its allocation
 void launch_expected_depths_dead(b200_engine *e, const SceneRef &s, int w, int h, b200_vec2f *minmax);
+// sweep != nullptr: the raycast's grid also runs that partial Decay's sweep, on CTAs of its own ahead of the ray tiles
 void launch_raycast(b200_engine *e, const SceneRef &s, const Mat4 &invM, const float proj[4], int w, int h, float voxelSize,
-                    float mu, const b200_vec2f *minmax, b200_vec4f *out, bool fused = false);
+                    float mu, const b200_vec2f *minmax, b200_vec4f *out, bool fused = false, const DecaySweep *sweep = nullptr);
 void launch_shade(b200_engine *e, const SceneRef &s, const Mat4 &M, const Mat4 &invM, int w, int h, float voxelSize, int maxW,
                   const b200_vec4f *rays, b200_vec4u *outChar, float *outDepth, int type);
 void launch_icp(b200_engine *e, const Mat4 &invM, int w, int h, float voxelSize, const b200_vec4f *rays, b200_vec4u *outImg,
@@ -207,7 +230,7 @@ static inline void trace_end(b200_engine *e, cudaStream_t st) {
 #define TRACED(e, st, name, ...) do { trace_begin(e, st, name); __VA_ARGS__; trace_end(e, st); } while (0)
 
 // Launch of a kernel of the fused frame's main-stream chain k_mark_prepare -> k_serve_list -> k_integrate_v4 -> k_raycast ->
-// k_decay_blocks<0>. With chained = true the launch carries programmatic stream serialisation: its CTAs may become resident and
+// k_decay_commit. With chained = true the launch carries programmatic stream serialisation: its CTAs may become resident and
 // run the code before their pdl_wait() while the previous kernel of the stream drains. Rules kept by every kernel of the chain:
 //  * a kernel calls pdl_trigger() only after its own pdl_wait() has returned. By induction, when a kernel runs its pre-wait code,
 //    everything two or more launches back has completed and its memory is visible;
@@ -215,6 +238,10 @@ static inline void trace_end(b200_engine *e, cudaStream_t st) {
 //    frame's first launch (k_mark_prepare, launched with chained = false, waits for everything enqueued before it);
 //  * pre-wait code writes only scratch that the previous kernel neither reads nor writes;
 //  * no stream operation (event record, copy, memset) sits between two chained launches: it would serialise them again.
+// The partial Decay's sweep runs on CTAs of k_raycast's grid, after the same wait. The rays read the voxels and the hash table
+// and write only the ray points, so the sweep may read the ring, the table and the voxels, and write only decay scratch that
+// nothing else in the grid touches: the delTag claims, itemPtr, resetPtr, the candidate list and the decay counters. The reset
+// stores and the table edits wait for k_decay_commit, launched after everything in the frame that reads the voxels.
 // Stand-alone entry points launch with chained = false; pdl_wait() is then a no-op and the kernels are unchanged.
 template <typename... KArgs, typename... Args>
 static inline void launch_chained(bool chained, void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t st,
@@ -230,7 +257,7 @@ static inline void launch_chained(bool chained, void (*kernel)(KArgs...), dim3 g
 
 // %globaltimer spans of the chain's kernels (b200_set_timing modes 2 to 4): one record of SPAN_KERNELS SpanStamp slots per fused
 // frame, SPAN_FRAMES records, zero-filled whenever the mode is set. Mode 2 stamps the integrate kernel only.
-enum { SPAN_MARK, SPAN_SERVE, SPAN_INTEGRATE, SPAN_RAYCAST, SPAN_DECAY, SPAN_KERNELS };
+enum { SPAN_MARK, SPAN_SERVE, SPAN_INTEGRATE, SPAN_RAYCAST, SPAN_SWEEP, SPAN_DECAY, SPAN_KERNELS };   // SPAN_RAYCAST: the ray CTAs only
 #define SPAN_FRAMES 8192
 // the slot of kernel k in the record of the fused frame being enqueued, or nullptr when that kernel is not stamped
 static inline unsigned long long *span_slot(const b200_engine *e, int k) {

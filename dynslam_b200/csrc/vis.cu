@@ -13,6 +13,7 @@
 // traced by 8x4-pixel warps so that a warp's rays walk the same voxel blocks; the voxel reads fetch
 // the 2-byte sdf only.
 #include "engine.h"
+#include "decay_sweep.cuh"
 #include "raycast_ray.cuh"
 #include "shade.cuh"
 #include <cstdlib>
@@ -275,10 +276,19 @@ template <bool useNbr>
 __global__ void __launch_bounds__(RC_THREADS)
 k_raycast(float4 *out, const b200_voxel *__restrict__ voxels, const b200_hash_entry *__restrict__ table, int nb, int w, int h, Mat4 invM,
           float fx, float fy, float cxp, float cyp, float voxelSize, float mu, const float2 *__restrict__ minmax, int twLog2, int centreRow,
-          int tilesX, int tilesY, unsigned tilesXMagic, unsigned long long *span) {
+          int tilesX, int tilesY, unsigned tilesXMagic, unsigned long long *span, DecaySweep sweep, int sweepCtas) {
+  if ((int)blockIdx.x < sweepCtas) {
+    // CTAs [0, sweepCtas): a partial Decay's sweep (decay_sweep.cuh), which reads what the rays read and writes only decay
+    // scratch (launch_chained's rules). Dispatched first, they take SM slots while the first waves of rays are issue-bound.
+    pdl_wait();
+    pdl_trigger();
+    SpanStamp stamp(sweep.span);
+    decay_sweep<0>(sweep, (blockIdx.x * RC_THREADS + threadIdx.x) >> 5, sweepCtas * (RC_THREADS / 32));
+    return;
+  }
   // warp tile: (1 << twLog2) x (32 >> twLog2) pixels
   const int tw = 1 << twLog2, th = 32 >> twLog2;
-  const int warpGlobal = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+  const int warpGlobal = ((blockIdx.x - sweepCtas) * blockDim.x + threadIdx.x) >> 5;
   if (warpGlobal >= tilesX * tilesY) return;
   const int lane = threadIdx.x & 31;
   const int rowLinear = (int)__umulhi((unsigned)warpGlobal, tilesXMagic);      // warpGlobal / tilesX (magic = ceil(2^32 / tilesX))
@@ -311,7 +321,7 @@ k_raycast(float4 *out, const b200_voxel *__restrict__ voxels, const b200_hash_en
 }
 
 void launch_raycast(b200_engine *e, const SceneRef &s, const Mat4 &invM, const float proj[4], int w, int h, float voxelSize, float mu,
-                    const b200_vec2f *minmax, b200_vec4f *out, bool fused) {
+                    const b200_vec2f *minmax, b200_vec4f *out, bool fused, const DecaySweep *sweep) {
   const int twLog2 = e->rcTileLog2;   // warp tile (1 << twLog2) x (32 >> twLog2) pixels; 3: 8x4 (default)
   const int tw = 1 << twLog2, th = 32 >> twLog2;
   const int tiles = ((w + tw - 1) / tw) * ((h + th - 1) / th);
@@ -326,10 +336,14 @@ void launch_raycast(b200_engine *e, const SceneRef &s, const Mat4 &invM, const f
   const int tilesXh = (w + tw - 1) / tw, tilesYh = (h + th - 1) / th;
   const unsigned magic = (unsigned)((0x100000000ull + (unsigned)tilesXh - 1) / (unsigned)tilesXh);
   const int impl = e->rcImpl;   // 1: neighbourhood cache (default); 0: per-lane one-entry cache (cross-check)
+  // The sweep's CTAs loop over the snapshot's items (a visible list, a few thousand blocks): 4 CTAs (8 warps) per SM, beside
+  // the 25 raycast CTAs an SM holds.
+  const int sweepCtas = sweep ? e->smCount * 4 : 0;
   trace_begin(e, e->stream, "k_raycast");
-  launch_chained(fused, impl ? k_raycast<true> : k_raycast<false>, (tiles + warpsPerCta - 1) / warpsPerCta, RC_THREADS, 0, e->stream,
-                 (float4 *)out, s.voxels, s.hash, s.numBuckets, w, h, invM, proj[0], proj[1], proj[2], proj[3], voxelSize, mu,
-                 (const float2 *)minmax, twLog2, centreRow, tilesXh, tilesYh, magic, fused ? span_slot(e, SPAN_RAYCAST) : nullptr);
+  launch_chained(fused, impl ? k_raycast<true> : k_raycast<false>, sweepCtas + (tiles + warpsPerCta - 1) / warpsPerCta, RC_THREADS, 0,
+                 e->stream, (float4 *)out, s.voxels, s.hash, s.numBuckets, w, h, invM, proj[0], proj[1], proj[2], proj[3], voxelSize, mu,
+                 (const float2 *)minmax, twLog2, centreRow, tilesXh, tilesYh, magic, fused ? span_slot(e, SPAN_RAYCAST) : nullptr,
+                 sweep ? *sweep : DecaySweep{}, sweepCtas);
   trace_end(e, e->stream);
   e->launches++;
 }

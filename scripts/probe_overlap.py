@@ -3,8 +3,9 @@
 Runs the bench configuration (1242x375 KITTI-shaped stream, 0x60000 blocks, 0x100000 + 0x80000 entries, decay maxWeight 1 /
 minAge 200, 230-frame pre-roll so partial decay is live, L2 flushed before every frame) and reads the kernels' own %globaltimer
 stamps (b200_set_timing(4), b200_diag_read_spans): per kernel the first CTA's entry after its dependency wait and the last warp's
-exit. Prints, as medians over the measured frames, each kernel's span, the idle time at each of the four boundaries (next
-entry - previous exit) and the frame's chain from the first entry to the last exit.
+exit. The partial decay's sweep runs on CTAs of its own inside the raycast's grid and is stamped apart from the ray CTAs;
+the raycast launch's span covers both. Prints, as medians over the measured frames, each span, the idle time at each of the
+four boundaries between launches (next entry - previous exit) and the frame's chain from the first entry to the last exit.
 
 Then mode 3 (an event pair around every launch, which serialises the chain) for the same number of frames: the integrate
 kernel's stamp span against its event pair, launch by launch — the check that the stamps time the integrate launch as the
@@ -18,7 +19,8 @@ import numpy as np, torch
 from dynslam_b200 import engine as E, synth
 import bench
 
-NAMES = ["k_mark_prepare", "k_serve_list", "k_integrate", "k_raycast", "k_decay_blocks<0>"]
+NAMES = ["k_mark_prepare", "k_serve_list", "k_integrate", "k_raycast", "decay sweep", "k_decay_commit"]   # b200_diag_read_spans' slots
+CHAIN = ["k_mark_prepare", "k_serve_list", "k_integrate", "k_raycast launch", "k_decay_commit"]             # the launches, in order
 
 
 def read_spans(eng, n):
@@ -68,16 +70,24 @@ def main():
     sp = sp[ok]
     us = lambda a: float(np.median(a)) / 1000.0
     spans = {NAMES[k]: us(sp[:, k, 1] - sp[:, k, 0]) for k in range(len(NAMES))}
-    gaps = {f"{NAMES[k]} -> {NAMES[k + 1]}": us(sp[:, k + 1, 0] - sp[:, k, 1]) for k in range(len(NAMES) - 1)}
-    chain = us(sp[:, -1, 1] - sp[:, 0, 0])
-    out.update({"frames": int(ok.sum()), "span_us": spans, "idle_us": gaps, "chain_us": chain,
-                "sum_of_spans_us": sum(spans.values()), "sum_of_idle_us": sum(gaps.values())})
+    rc, sw = NAMES.index("k_raycast"), NAMES.index("decay sweep")
+    launch = np.stack([np.minimum(sp[:, rc, 0], sp[:, sw, 0]), np.maximum(sp[:, rc, 1], sp[:, sw, 1])], axis=1)
+    ch = np.stack([sp[:, 0], sp[:, 1], sp[:, 2], launch, sp[:, NAMES.index("k_decay_commit")]], axis=1)
+    chain_spans = {CHAIN[k]: us(ch[:, k, 1] - ch[:, k, 0]) for k in range(len(CHAIN))}
+    gaps = {f"{CHAIN[k]} -> {CHAIN[k + 1]}": us(ch[:, k + 1, 0] - ch[:, k, 1]) for k in range(len(CHAIN) - 1)}
+    chain = us(ch[:, -1, 1] - ch[:, 0, 0])
+    out.update({"frames": int(ok.sum()), "span_us": spans, "launch_span_us": chain_spans, "idle_us": gaps, "chain_us": chain,
+                "sum_of_spans_us": sum(chain_spans.values()), "sum_of_idle_us": sum(gaps.values()),
+                "sweep_entry_after_raycast_entry_us": us(sp[:, sw, 0] - sp[:, rc, 0]),
+                "sweep_exit_before_raycast_exit_us": us(sp[:, rc, 1] - sp[:, sw, 1])})
     print(f"device {props.name}; {int(ok.sum())} frames with every kernel stamped (medians, us)")
     for k, v in spans.items():
         print(f"  span  {k:<20s} {v:7.2f}")
+    print(f"  span  {'k_raycast launch':<20s} {chain_spans['k_raycast launch']:7.2f}   (ray CTAs and sweep CTAs)")
+    print(f"  sweep exit before the last ray exit {out['sweep_exit_before_raycast_exit_us']:7.2f}")
     for k, v in gaps.items():
         print(f"  idle  {k:<40s} {v:7.2f}   (negative: the next kernel's first CTA passed its wait before the last warp left)")
-    print(f"  chain first entry -> last exit {chain:7.2f}; spans {sum(spans.values()):.2f} + idle {sum(gaps.values()):.2f}")
+    print(f"  chain first entry -> last exit {chain:7.2f}; launch spans {sum(chain_spans.values()):.2f} + idle {sum(gaps.values()):.2f}")
 
     # ---- mode 3: the integrate kernel's stamps against an event pair around each launch (no overlap: events in the chain) ----
     views = [view(frames[idx + i]) for i in range(n)]; idx += n
