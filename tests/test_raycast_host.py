@@ -11,6 +11,7 @@ import pytest
 
 from dynslam_b200 import abi, synth
 from tests import hostlib as H
+from tests import poselib as PL
 
 HERE = os.path.join(os.path.dirname(os.path.abspath(__file__)), "hostcheck")
 
@@ -53,3 +54,31 @@ def test_cast_ray_equals_oracle(lib, voxel, mu, nbuckets, frames):
             hit = int((out[..., 3] > 0).sum())
             assert hit > w * h // 4
             assert out.tobytes() == vol.raycastResult.tobytes(), variant
+
+
+@pytest.mark.parametrize("name", PL.NAMES)
+def test_cast_ray_general_poses_equals_oracle(lib, name):
+    """the general-pose trajectories of tests/poselib.py: negative and far-from-zero block coordinates, rays marching in every
+    direction through the block-neighbourhood cache (per-axis carries and re-keying at block boundaries both ways), fx != fy,
+    off-centre and off-image principal points. Rendered from the last pose and from the last camera turned 35 and 90 degrees."""
+    L, t = H.oracle(), PL.get(name)
+    nb = 0x2000
+    vol = H.HostVolume(16384, nb, 0x4000, t.w, t.h, H.SceneParams(PL.VOXEL, t.mu, 50, 0.1, 300.0, 0))
+    for depth, rgb, M, proj in t.frames():
+        hv = H.make_view(depth, rgb, M, proj)
+        assert L.oracle_allocate_from_depth(vol.engine, C.byref(vol.scene), C.byref(vol.rs), C.byref(hv), 0, 0) == 0
+        L.oracle_integrate(vol.engine, C.byref(vol.scene), C.byref(vol.rs), C.byref(hv), 0)
+    hits = []
+    for Mv in (M, t.turned(35.0), t.turned(90.0)):
+        hv = H.make_view(depth, rgb, Mv, t.proj)
+        cam = H.make_camera(Mv, t.proj)
+        L.oracle_find_visible_blocks(C.byref(vol.scene), C.byref(vol.rs), C.byref(cam))
+        L.oracle_expected_depths(C.byref(vol.scene), C.byref(vol.rs), C.byref(cam))
+        L.oracle_icp_maps(C.byref(vol.scene), C.byref(vol.rs), C.byref(hv), H.vptr(vol.points), H.vptr(vol.normals), 0)
+        for variant in (0, 1):
+            out = np.zeros((t.h, t.w, 4), np.float32)
+            lib.hostcheck_raycast(H.vptr(vol.voxels), H.vptr(vol.hash), nb, t.w, t.h, hv.invM_d, hv.proj_d, PL.VOXEL, t.mu,
+                                  H.vptr(vol.minmax), H.vptr(out), variant)
+            assert out.tobytes() == vol.raycastResult.tobytes(), (name, variant)
+        hits.append(int((vol.raycastResult[..., 3] > 0).sum()))
+    assert hits[0] > t.w * t.h // 3, hits
