@@ -186,7 +186,7 @@ EXPORTS = [
     "b200_render_view_async", "b200_render_view_sync", "b200_render_view_submit", "b200_render_view_wait", "b200_engine_wait_engine",
 ]
 # measurement / test hooks (include/b200fusion_diag.h): exported by the same library, not part of the drop-in boundary
-DIAG_EXPORTS = ["b200_set_timing", "b200_get_trace", "b200_get_stats", "b200_selftest_divide", "b200_diag_set_max_rendering_blocks",
+DIAG_EXPORTS = ["b200_set_timing", "b200_get_trace", "b200_get_stats", "b200_selftest_divide", "b200_diag_set_max_rendering_blocks", "b200_diag_set_grid_scale",
                 "b200_diag_read_debug", "b200_diag_read_spans", "b200_diag_last_integrate", "b200_diag_push_decay_snapshot", "b200_diag_set_frame_index"]
 
 _lib = None
@@ -277,6 +277,8 @@ def load_library():
     lib.b200_selftest_divide.argtypes = [vp, C.c_uint64, C.c_uint64, C.c_float, P(C.c_uint64)]
     lib.b200_diag_set_max_rendering_blocks.argtypes = [vp, C.c_int]
     lib.b200_diag_set_max_rendering_blocks.restype = None
+    lib.b200_diag_set_grid_scale.argtypes = [vp, C.c_int]
+    lib.b200_diag_set_grid_scale.restype = None
     lib.b200_diag_read_debug.argtypes = [vp, P(C.c_uint64), C.c_int]
     lib.b200_diag_read_spans.argtypes = [vp, P(C.c_uint64), C.c_int]
     lib.b200_diag_read_spans.restype = C.c_int

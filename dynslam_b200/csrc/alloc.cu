@@ -320,9 +320,13 @@ DEV unsigned nz_bytes(unsigned w) { return ((__vcmpne4(w, 0u) & 0x80808080u) * 0
 // CreateExpectedDepths renders from this very pose — ProjectSingleBlock and the rasterisation of the block's 1/8-resolution
 // box into the expected-depth image with atomic min / max on the (positive) float bit patterns. The listed entries of a
 // tile are dealt round-robin to its eight warps.
-// A new excess-list entry lies in another tile than the request that creates it: tiles of the excess part of the table
-// start phase B only when every tile has finished phase A (device-wide counter; the grid is persistent and co-resident, and
-// a CTA finishes phase A of ALL its tiles before it starts phase B of any).
+// A new excess-list entry lies in another tile than the request that creates it: in a frame with excess-list requests, the
+// tiles of the excess part of the table (the last ones) start phase B only when every tile has finished phase A (device-wide
+// counter). Tiles are drawn from two tickets (draw_tile, common.cuh), so that no CTA waits on a tile nobody has claimed:
+//  * the first ticket deals every tile for phase A and, unless the tile is deferred, phase B right after it. Phase B of an
+//    ordered tile waits only on lower tiles (the look-back), all claimed and never deferred;
+//  * the second deals phase B of the deferred tiles. A CTA draws from it only after the first ticket has run out, so when it
+//    waits for all of phase A, every tile's phase A is owned by a running CTA that waits on nothing but lower tiles' phase A.
 // ------------------------------------------------------------------------------------------------
 #define AL_EPT 32
 #define AL_TILE (256 * AL_EPT)   // 8192 entries = 256 bitmap words per tile
@@ -330,6 +334,7 @@ DEV unsigned nz_bytes(unsigned w) { return ((__vcmpne4(w, 0u) & 0x80808080u) * 0
 
 #define AL_GROUP_BOX 64          // live cells up to which the entry's 8-lane group rasterises the box
 
+template <bool TICKETED>
 __global__ void __launch_bounds__(256, 2)
 k_serve_list(const float *__restrict__ depth, b200_hash_entry *table, int numBuckets, int noTotal, uint8_t *visType,
              const unsigned long long *__restrict__ reqKey, unsigned *reqBits, unsigned *req2Bits, uint8_t *markBytes,
@@ -353,237 +358,297 @@ k_serve_list(const float *__restrict__ depth, b200_hash_entry *table, int numBuc
   const int noWords = noTotal >> 5;
   const int noTiles = (noTotal + AL_TILE - 1) / AL_TILE;
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  // One pass (every tile: requests, then its list) when each CTA owns a single tile — the usual case: 192 tiles for the
-  // default table — so that a tile's list count is published before anybody serves a request and nobody waits on a serving
-  // tile. Two passes (all requests first) when CTAs own several tiles: a tile of the excess part may have to wait for every
-  // tile's requests, including those this very CTA still has to serve.
-  const bool twoPass = noTiles > (int)gridDim.x;
   // the marking kernel says whether ANY excess-list request was filed this frame: only then can a tile of the excess part
   // receive an entry (and a visibility mark) from another tile's service, and has to wait for all of them
   const bool anyExcess = !onlyVisible && *(volatile int *)&ctr->anyExcessRequest != 0;
-  const int baseVba = ctr->lastFreeBlockId, baseExl = ctr->lastFreeExcessListId;   // only the last tile updates them
+  // Read at entry and changed by the last tile only, by the CTA that serves (baseVba, baseExl) or lists (ringStart) it: that
+  // CTA read them before. (In the ticketed form a CTA that starts later finds the tickets drained and uses neither.)
+  const int baseVba = ctr->lastFreeBlockId, baseExl = ctr->lastFreeExcessListId;
+  const long long ringStart = ctr->ringHead;
   const float invfx = 1.0f / g.proj_d[0], invfy = 1.0f / g.proj_d[1];
   const float oneOverVoxelSize = 1.0f / (g.voxelSize * BS);
-  const long long ringStart = ctr->ringHead;   // advanced by the last tile only, at its very end
   const int liveX = (rw - 1) / B200_MINMAX_SUBSAMPLE, liveY = (rh - 1) / B200_MINMAX_SUBSAMPLE;   // last live cell of the expected-depth image
   unsigned long long *const dAB[2] = {descA, descB};
   unsigned long long *const dC[1] = {descC};
   unsigned myTiles = 0;   // rendering tiles of the blocks this thread projected (fused frame only)
-
-  const long long ringBase = ringStart % ringCap;   // one 64-bit division per thread instead of one per listed entry
   const int grp = warp * 4 + (lane >> 3), sub = lane & 7;   // hit phase: an 8-lane group per listed entry, one lane per block corner
-  for (int pass = 0; pass < (twoPass ? 2 : 1); ++pass) {
-    const bool doReq = !twoPass || pass == 0, doList = !twoPass || pass == 1;
-    for (int tile = blockIdx.x; tile < noTiles; tile += gridDim.x) {
-      const int first = tile * AL_TILE + threadIdx.x * AL_EPT;
-      const int w = tile * 256 + threadIdx.x;
-      const bool last = (tile == noTiles - 1);
-      const bool deferList = anyExcess && ((tile + 1) * AL_TILE > numBuckets);   // its new children arrive from other tiles' service
-      K2_TILE_STAMP(0, tile);
-      // ---- every load of the tile is issued up front: request words, the first request's key, visibility and mark bytes ----
-      unsigned rq = 0, rq2 = 0, localPacked = 0, total = 0, total2 = 0;
-      unsigned long long key0 = 0ull;
-      uint4 raw[2], mb[2];
-      raw[0] = raw[1] = mb[0] = mb[1] = make_uint4(0u, 0u, 0u, 0u);
-      if (w < noWords) {
-        if (doReq) { rq = reqBits[w]; rq2 = req2Bits[w]; }
-        if (doList) {
-          raw[0] = __ldcg(reinterpret_cast<const uint4 *>(visType + first));          // noTotal is a multiple of 32
-          raw[1] = __ldcg(reinterpret_cast<const uint4 *>(visType + first + 16));
-          mb[0] = __ldcg(reinterpret_cast<const uint4 *>(markBytes + first));         // written by the marking kernel and by other tiles' service: L2
-          mb[1] = __ldcg(reinterpret_cast<const uint4 *>(markBytes + first + 16));
-        }
+
+  // ---- the steps of one tile (a CTA works on one tile at a time; both forms below run them in their own order) ----
+  int first = 0, w = 0;
+  bool last = false;
+  unsigned rq = 0, rq2 = 0, localPacked = 0, total = 0, total2 = 0, mask = 0, mk = 0, local = 0, totalC = 0;
+  unsigned long long key0 = 0ull;
+  uint4 raw[2], mb[2];
+  // every load of the tile is issued up front: request words, visibility and mark bytes
+  auto load_tile = [&](int tile, bool doReq, bool doList) {
+    first = tile * AL_TILE + threadIdx.x * AL_EPT;
+    w = tile * 256 + threadIdx.x;
+    last = (tile == noTiles - 1);
+    rq = rq2 = localPacked = total = total2 = mask = mk = local = totalC = 0;
+    key0 = 0ull;
+    raw[0] = raw[1] = mb[0] = mb[1] = make_uint4(0u, 0u, 0u, 0u);
+    if (w < noWords) {
+      if (doReq) { rq = reqBits[w]; rq2 = req2Bits[w]; }
+      if (doList) {
+        raw[0] = __ldcg(reinterpret_cast<const uint4 *>(visType + first));          // noTotal is a multiple of 32
+        raw[1] = __ldcg(reinterpret_cast<const uint4 *>(visType + first + 16));
+        mb[0] = __ldcg(reinterpret_cast<const uint4 *>(markBytes + first));         // written by the marking kernel and by other tiles' service: L2
+        mb[1] = __ldcg(reinterpret_cast<const uint4 *>(markBytes + first + 16));
       }
-      // ---- requests: rank (published at once), serve later ----
-      if (doReq) {
-        if (w < noWords) {
-          if (rq) reqBits[w] = 0u;                 // consumed: clean for the next frame
-          if (rq2) req2Bits[w] = 0u;
-        }
-        if (onlyVisible) { rq = 0u; rq2 = 0u; }     // onlyUpdateVisibleList: the marking ran, nothing is allocated (Reco_CUDA.cu:254-262)
-        if (rq) key0 = reqKey[w * 32 + __ffs(rq) - 1];
-        unsigned totalPacked;
-        localPacked = block_exclusive_scan(__popc(rq) | (__popc(rq2) << 16), sm, &totalPacked);   // <= 8192 each: no carry
-        total = totalPacked & 0xffffu; total2 = totalPacked >> 16;
-        if (threadIdx.x < 32) { const unsigned agg[2] = {total, total2}; lookback_publish<2>(dAB, gen, tile, agg); }
-        if (threadIdx.x == 0) {
-          if (total2) atomicAdd(&ctr->tilesWithExcess, 1u);
-          __threadfence();
-          atomicAdd(&ctr->tilesRanked, 1u);         // after the count above: tilesRanked == noTiles makes tilesWithExcess final
-        }
-      }
-      // ---- list, first half: visibility bytes -> mask of listed entries, count published ----
-      unsigned mask = 0, mk = 0, local = 0, totalC = 0;
-      auto decode = [&](const bool marksOnly, const bool clearMarks) {
-        // Byte-parallel (four entries per 32-bit operation, no loop over the interesting bytes): the excess part of the table
-        // is dense — every listed excess entry of a KITTI frame sits in the last tile, a dozen per thread — and a per-byte
-        // loop there was the longest chain of the launch.
-        if (w < noWords) {
+    }
+  };
+  auto reload_marks = [&]() {
+    if (w < noWords) {
+      mb[0] = __ldcg(reinterpret_cast<const uint4 *>(markBytes + first));
+      mb[1] = __ldcg(reinterpret_cast<const uint4 *>(markBytes + first + 16));
+    }
+  };
+  // requests, first half: rank counts published at once (the first request's key is fetched here too)
+  auto rank_publish = [&](int tile) {
+    if (w < noWords) {
+      if (rq) reqBits[w] = 0u;                 // consumed: clean for the next frame
+      if (rq2) req2Bits[w] = 0u;
+    }
+    if (onlyVisible) { rq = 0u; rq2 = 0u; }     // onlyUpdateVisibleList: the marking ran, nothing is allocated (Reco_CUDA.cu:254-262)
+    if (rq) key0 = reqKey[w * 32 + __ffs(rq) - 1];
+    unsigned totalPacked;
+    localPacked = block_exclusive_scan(__popc(rq) | (__popc(rq2) << 16), sm, &totalPacked);   // <= 8192 each: no carry
+    total = totalPacked & 0xffffu; total2 = totalPacked >> 16;
+    if (threadIdx.x < 32) { const unsigned agg[2] = {total, total2}; lookback_publish<2>(dAB, gen, tile, agg); }
+  };
+  // list, first half: visibility bytes -> mask of listed entries. Byte-parallel (four entries per 32-bit operation, no loop over
+  // the interesting bytes): the excess part of the table is dense — every listed excess entry of a KITTI frame sits in the last
+  // tile, a dozen per thread — and a per-byte loop there was the longest chain of the launch.
+  auto decode = [&](const bool marksOnly, const bool clearMarks) {
+    if (w < noWords) {
 #pragma unroll
-          for (int q = 0; q < 2; ++q) {
-            const unsigned mw[4] = {mb[q].x, mb[q].y, mb[q].z, mb[q].w};
-            unsigned xv[4] = {raw[q].x, raw[q].y, raw[q].z, raw[q].w};
-            if ((mw[0] | mw[1] | mw[2] | mw[3]) && clearMarks) *reinterpret_cast<uint4 *>(markBytes + first + q * 16) = make_uint4(0u, 0u, 0u, 0u);   // consumed
-            bool dirty = false;
+      for (int q = 0; q < 2; ++q) {
+        const unsigned mw[4] = {mb[q].x, mb[q].y, mb[q].z, mb[q].w};
+        unsigned xv[4] = {raw[q].x, raw[q].y, raw[q].z, raw[q].w};
+        if ((mw[0] | mw[1] | mw[2] | mw[3]) && clearMarks) *reinterpret_cast<uint4 *>(markBytes + first + q * 16) = make_uint4(0u, 0u, 0u, 0u);   // consumed
+        bool dirty = false;
 #pragma unroll
-            for (int j = 0; j < 4; ++j) {
-              const unsigned markM = __vcmpne4(mw[j], 0u);      // 0xff where the entry was observed this frame
-              const unsigned x = xv[j];
-              unsigned nv;
-              if (marksOnly) nv = (x & ~markM) | (markM & 0x01010101u);
-              else {
-                const unsigned pvM = __vcmpeq4(x, VT_PREV_VISIBLE * 0x01010101u) & ~markM, phM = __vcmpeq4(x, VT_PREV_HIDDEN * 0x01010101u) & ~markM;
-                // observed -> 1 (2 = swapped out is patched where the entry is read); previous list: re-tested visible -> 3, hidden -> 0
-                nv = (x & ~(markM | pvM | phM)) | (markM & 0x01010101u) | (pvM & 0x03030303u);
-                unsigned st = __vcmpeq4(x, 0x03030303u) & ~markM & 0x80808080u;      // a 3 the prepare pass did not re-test (list overflow): rare
-                while (st) {
-                  const int byte = (__ffs(st) - 1) >> 3;
-                  st &= st - 1;
-                  if (!stale_three_visible(table, first + q * 16 + j * 4 + byte, &g)) nv &= ~(0xffu << (byte * 8));
-                }
-              }
-              if (nv != x) { dirty = true; xv[j] = nv; }
-              mask |= nz_bytes(nv) << (q * 16 + j * 4);
-              mk |= nz_bytes(mw[j]) << (q * 16 + j * 4);
-            }
-            if (dirty) {
-              raw[q] = make_uint4(xv[0], xv[1], xv[2], xv[3]);
-              *reinterpret_cast<uint4 *>(visType + first + q * 16) = raw[q];
+        for (int j = 0; j < 4; ++j) {
+          const unsigned markM = __vcmpne4(mw[j], 0u);      // 0xff where the entry was observed this frame
+          const unsigned x = xv[j];
+          unsigned nv;
+          if (marksOnly) nv = (x & ~markM) | (markM & 0x01010101u);
+          else {
+            const unsigned pvM = __vcmpeq4(x, VT_PREV_VISIBLE * 0x01010101u) & ~markM, phM = __vcmpeq4(x, VT_PREV_HIDDEN * 0x01010101u) & ~markM;
+            // observed -> 1 (2 = swapped out is patched where the entry is read); previous list: re-tested visible -> 3, hidden -> 0
+            nv = (x & ~(markM | pvM | phM)) | (markM & 0x01010101u) | (pvM & 0x03030303u);
+            unsigned st = __vcmpeq4(x, 0x03030303u) & ~markM & 0x80808080u;      // a 3 the prepare pass did not re-test (list overflow): rare
+            while (st) {
+              const int byte = (__ffs(st) - 1) >> 3;
+              st &= st - 1;
+              if (!stale_three_visible(table, first + q * 16 + j * 4 + byte, &g)) nv &= ~(0xffu << (byte * 8));
             }
           }
+          if (nv != x) { dirty = true; xv[j] = nv; }
+          mask |= nz_bytes(nv) << (q * 16 + j * 4);
+          mk |= nz_bytes(mw[j]) << (q * 16 + j * 4);
         }
-      };
-      auto count_and_publish = [&]() {
-        local = block_exclusive_scan(__popc(mask), sm, &totalC);
-        if (threadIdx.x < 32) { const unsigned agg[1] = {totalC}; lookback_publish<1>(dC, gen, tile, agg); }
-        K2_TILE_STAMP(1, tile);
-        if (dbg && threadIdx.x == 0 && tile < 1024) dbg[64 + 3 * 1024 + tile] = totalC;
-      };
-      K2_STAMP(1);
-      // The list count of a tile never depends on the tile's OWN service (the marking kernel already marked the ordered entries
-      // it requested; children land in the excess part), so it is published before anybody serves anything: no tile of the
-      // ordered part ever waits for a serving tile. (A tile that still waits for other tiles' child marks leaves the mark bytes
-      // alone in this early pass: clearing a 16-byte group here could wipe a mark another tile is writing into it right now.)
-      if (doList) { decode(false, !deferList); if (!deferList) count_and_publish(); }
-      K2_STAMP(2);
-      // ---- requests, second half: ranks of this tile's requests (and the grand totals on the last tile), service ----
-      if (doReq) {
-        const bool needRank = (total != 0) || last;
-        if (needRank && threadIdx.x < 32) {
-          const unsigned agg[2] = {total, total2};
-          unsigned ex[2];
-          lookback_walk<2>(dAB, gen, tile, agg, ex);
-          if (threadIdx.x == 0) { tileBase = ex[0]; tileBase2 = ex[1]; }
-        }
-        __syncthreads();
-        if (needRank) {
-          unsigned rank = tileBase + (localPacked & 0xffffu), rank2 = tileBase2 + (localPacked >> 16);
-          const unsigned grand = tileBase + total, grand2 = tileBase2 + total2;
-          bool firstReq = true;
-          while (rq) {
-            const int b = __ffs(rq) - 1;
-            rq &= rq - 1;
-            const int targetIdx = w * 32 + b;
-            const bool isExcess = (rq2 >> b) & 1u;
-            const int vbaIdx = baseVba - (int)rank;
-            const int exlIdx = baseExl - (int)rank2;
-            rank++;
-            if (isExcess) rank2++;
-            const unsigned long long key = firstReq ? key0 : reqKey[targetIdx];
-            firstReq = false;
-            if (vbaIdx < 0 || (isExcess && exlIdx < 0)) continue;   // exhausted: the counters still go negative
-            const unsigned step = (unsigned)(key & ((1u << KEY_STEP_BITS) - 1));
-            const unsigned pixel = (unsigned)((key >> KEY_STEP_BITS) & ((1u << KEY_PIXEL_BITS) - 1));
-            const int x = pixel % g.w, y = pixel / g.w;
-            Ray r;
-            make_ray(r, x, y, __ldg(depth + pixel), g, invfx, invfy, oneOverVoxelSize);
-            float px = r.px, py = r.py, pz = r.pz;
-            for (unsigned i = 0; i < step; ++i) { px += r.dx; py += r.dy; pz += r.dz; }
-            const int bx = (short)(int)floorf(px), by = (short)(int)floorf(py), bz = (short)(int)floorf(pz);
-            int *ew;
-            if (!isExcess) {
-              ew = reinterpret_cast<int *>(table) + (size_t)targetIdx * 5;
-            } else {
-              const int exlOffset = excessList[exlIdx];
-              reinterpret_cast<int *>(table)[(size_t)targetIdx * 5 + 2] = exlOffset + 1;   // connect to child
-              ew = reinterpret_cast<int *>(table) + (size_t)(numBuckets + exlOffset) * 5;
-              markBytes[numBuckets + exlOffset] = 1;                                       // child visible (:875)
-            }
-            ew[0] = (int)(((unsigned)bx & 0xffffu) | ((unsigned)by << 16));
-            ew[1] = (bz & 0xffff);
-            ew[2] = 0;
-            ew[3] = allocList[vbaIdx];
-            ew[4] = currentFrame;
-          }
-          if (last && threadIdx.x == 0) {
-            ctr->allocBaseVba = baseVba; ctr->allocBaseExl = baseExl;
-            ctr->noRequests = (int)grand; ctr->noRequestsExcess = (int)grand2;
-            ctr->lastFreeBlockId = baseVba - (int)grand;
-            ctr->lastFreeExcessListId = baseExl - (int)grand2;
-          }
-        }
-        __syncthreads();             // the hit phase below reads entries this tile's service wrote
-        if (total2 != 0 && threadIdx.x == 0) {
-          __threadfence();                              // this tile's new child entries and their marks are visible device-wide ...
-          atomicAdd(&ctr->tilesExcessServed, 1u);       // ... before it counts as served
+        if (dirty) {
+          raw[q] = make_uint4(xv[0], xv[1], xv[2], xv[3]);
+          *reinterpret_cast<uint4 *>(visType + first + q * 16) = raw[q];
         }
       }
-      K2_STAMP(3);
-      K2_TILE_STAMP(4, tile);
-      if (!doList) continue;
-      // ---- list, late part of the first half: a tile of the excess part in a frame with excess requests ----
-      if (deferList) {
-        // everything but this frame's new children is decoded already; wait until every tile with excess requests has
-        // served them (their number is final once all tiles have published their counts), then pick up the new marks
-        if (threadIdx.x == 0) {
-          while (*(volatile unsigned *)&ctr->tilesRanked < (unsigned)noTiles) { }
-          const unsigned need = *(volatile unsigned *)&ctr->tilesWithExcess;
-          while (*(volatile unsigned *)&ctr->tilesExcessServed < need) { }
-          __threadfence();
+    }
+  };
+  auto count_and_publish = [&](int tile) {
+    local = block_exclusive_scan(__popc(mask), sm, &totalC);
+    if (threadIdx.x < 32) { const unsigned agg[1] = {totalC}; lookback_publish<1>(dC, gen, tile, agg); }
+    K2_TILE_STAMP(1, tile);
+    if (dbg && threadIdx.x == 0 && tile < 1024) dbg[64 + 3 * 1024 + tile] = totalC;
+  };
+  // requests, second half: ranks of this tile's requests (and the grand totals on the last tile), service
+  auto serve = [&](int tile) {
+    const bool needRank = (total != 0) || last;
+    if (needRank && threadIdx.x < 32) {
+      const unsigned agg[2] = {total, total2};
+      unsigned ex[2];
+      lookback_walk<2>(dAB, gen, tile, agg, ex);
+      if (threadIdx.x == 0) { tileBase = ex[0]; tileBase2 = ex[1]; }
+    }
+    __syncthreads();
+    if (needRank) {
+      unsigned rank = tileBase + (localPacked & 0xffffu), rank2 = tileBase2 + (localPacked >> 16);
+      const unsigned grand = tileBase + total, grand2 = tileBase2 + total2;
+      bool firstReq = true;
+      while (rq) {
+        const int b = __ffs(rq) - 1;
+        rq &= rq - 1;
+        const int targetIdx = w * 32 + b;
+        const bool isExcess = (rq2 >> b) & 1u;
+        const int vbaIdx = baseVba - (int)rank;
+        const int exlIdx = baseExl - (int)rank2;
+        rank++;
+        if (isExcess) rank2++;
+        const unsigned long long key = firstReq ? key0 : reqKey[targetIdx];
+        firstReq = false;
+        if (vbaIdx < 0 || (isExcess && exlIdx < 0)) continue;   // exhausted: the counters still go negative
+        const unsigned step = (unsigned)(key & ((1u << KEY_STEP_BITS) - 1));
+        const unsigned pixel = (unsigned)((key >> KEY_STEP_BITS) & ((1u << KEY_PIXEL_BITS) - 1));
+        const int x = pixel % g.w, y = pixel / g.w;
+        Ray r;
+        make_ray(r, x, y, __ldg(depth + pixel), g, invfx, invfy, oneOverVoxelSize);
+        float px = r.px, py = r.py, pz = r.pz;
+        for (unsigned i = 0; i < step; ++i) { px += r.dx; py += r.dy; pz += r.dz; }
+        const int bx = (short)(int)floorf(px), by = (short)(int)floorf(py), bz = (short)(int)floorf(pz);
+        int *ew;
+        if (!isExcess) {
+          ew = reinterpret_cast<int *>(table) + (size_t)targetIdx * 5;
+        } else {
+          const int exlOffset = excessList[exlIdx];
+          reinterpret_cast<int *>(table)[(size_t)targetIdx * 5 + 2] = exlOffset + 1;   // connect to child
+          ew = reinterpret_cast<int *>(table) + (size_t)(numBuckets + exlOffset) * 5;
+          markBytes[numBuckets + exlOffset] = 1;                                       // child visible (:875)
         }
-        __syncthreads();
-        if (w < noWords) {
-          mb[0] = __ldcg(reinterpret_cast<const uint4 *>(markBytes + first));
-          mb[1] = __ldcg(reinterpret_cast<const uint4 *>(markBytes + first + 16));
-        }
-        decode(true, true);
-        count_and_publish();
-      }
-      // ---- list, second half: global offset; the listed entries go to their places in the list ----
-      if (threadIdx.x < 32) {
-        unsigned ex[1] = {0};
-        if (totalC != 0 || last) { const unsigned agg[1] = {totalC}; lookback_walk<1>(dC, gen, tile, agg, ex); }
-        if (threadIdx.x == 0) tileBase = ex[0];
-        K2_TILE_STAMP(2, tile);
-      }
-      __syncthreads();
-      K2_STAMP(4);
-      {
-        // the ptr list doubles as the hand-over: entry index | bit 31 (observed this frame) now, the block's ptr after the
-        // entry has been read (below, by whichever CTA gets the item)
-        long long o = (long long)tileBase + local;
-        while (mask) {
-          const int k = __ffs(mask) - 1;
-          mask &= mask - 1;
-          if (o < capacity) reinterpret_cast<unsigned *>(visiblePtr)[o] = (unsigned)(first + k) | (((mk >> k) & 1u) << 31);
-          ++o;
-        }
+        ew[0] = (int)(((unsigned)bx & 0xffffu) | ((unsigned)by << 16));
+        ew[1] = (bz & 0xffff);
+        ew[2] = 0;
+        ew[3] = allocList[vbaIdx];
+        ew[4] = currentFrame;
       }
       if (last && threadIdx.x == 0) {
-        const int n = (int)(tileBase + totalC);
-        ctr->noVisibleBlocks = n;
-        ctr->noIntegrated = 0;            // IntegrateIntoScene of this frame counts from zero (no separate memset)
-        const int kept = n < capacity ? n : capacity;
-        // (a snapshot that wraps onto older live ones simply overwrites them: decay.cu recognises an overwritten snapshot by
-        // ringHead - snapStart > ringCap when its turn comes and sweeps nothing — the oldest snapshots are dropped, never an error)
-        publish_snapshot(ctr, snapStart, snapCount, slot, ringStart, kept);
+        ctr->allocBaseVba = baseVba; ctr->allocBaseExl = baseExl;
+        ctr->noRequests = (int)grand; ctr->noRequestsExcess = (int)grand2;
+        ctr->lastFreeBlockId = baseVba - (int)grand;
+        ctr->lastFreeExcessListId = baseExl - (int)grand2;
       }
-      __syncthreads();
-      if (threadIdx.x == 0) {
-        __threadfence();                         // this tile's items (and, on the last tile, the total) are visible device-wide ...
-        atomicAdd(&ctr->tilesListed, 1u);        // ... before the tile counts as listed
+    }
+    __syncthreads();             // the hit phase below reads entries this tile's service wrote
+  };
+  // list, second half: global offset; the listed entries go to their places in the list
+  auto list_out = [&](int tile) {
+    if (threadIdx.x < 32) {
+      unsigned ex[1] = {0};
+      if (totalC != 0 || last) { const unsigned agg[1] = {totalC}; lookback_walk<1>(dC, gen, tile, agg, ex); }
+      if (threadIdx.x == 0) tileBase = ex[0];
+      K2_TILE_STAMP(2, tile);
+    }
+    __syncthreads();
+    K2_STAMP(4);
+    {
+      // the ptr list doubles as the hand-over: entry index | bit 31 (observed this frame) now, the block's ptr after the
+      // entry has been read (below, by whichever CTA gets the item)
+      long long o = (long long)tileBase + local;
+      while (mask) {
+        const int k = __ffs(mask) - 1;
+        mask &= mask - 1;
+        if (o < capacity) reinterpret_cast<unsigned *>(visiblePtr)[o] = (unsigned)(first + k) | (((mk >> k) & 1u) << 31);
+        ++o;
       }
-      K2_STAMP(5);
+    }
+    if (last && threadIdx.x == 0) {
+      const int n = (int)(tileBase + totalC);
+      ctr->noVisibleBlocks = n;
+      ctr->noIntegrated = 0;            // IntegrateIntoScene of this frame counts from zero (no separate memset)
+      const int kept = n < capacity ? n : capacity;
+      // (a snapshot that wraps onto older live ones simply overwrites them: decay.cu recognises an overwritten snapshot by
+      // ringHead - snapStart > ringCap when its turn comes and sweeps nothing — the oldest snapshots are dropped, never an error)
+      publish_snapshot(ctr, snapStart, snapCount, slot, ringStart, kept);
+    }
+    __syncthreads();
+    if (threadIdx.x == 0) {
+      __threadfence();                         // this tile's items (and, on the last tile, the total) are visible device-wide ...
+      atomicAdd(&ctr->tilesListed, 1u);        // ... before the tile counts as listed
+    }
+    K2_STAMP(5);
+  };
+  // The list count of an ordered tile never depends on the tile's OWN service (the marking kernel already marked the ordered
+  // entries it requested; children land in the excess part), so it is published before anybody serves anything: no tile of
+  // the ordered part ever waits for a serving tile.
+  if (!TICKETED) {
+    // CTA t owns tiles t, t + gridDim.x, ... One pass (every tile: requests, then its list) when each CTA owns a single tile —
+    // the usual case: 192 tiles for the default table — so that a tile's list count is published before anybody serves a
+    // request and nobody waits on a serving tile. Two passes (all requests first) when CTAs own several tiles: a tile of the
+    // excess part may have to wait for every tile's requests, including those this very CTA still has to serve.
+    const bool twoPass = noTiles > (int)gridDim.x;
+    for (int pass = 0; pass < (twoPass ? 2 : 1); ++pass) {
+      const bool doReq = !twoPass || pass == 0, doList = !twoPass || pass == 1;
+      for (int tile = blockIdx.x; tile < noTiles; tile += gridDim.x) {
+        const bool deferList = anyExcess && ((tile + 1) * AL_TILE > numBuckets);   // its new children arrive from other tiles' service
+        K2_TILE_STAMP(0, tile);
+        load_tile(tile, doReq, doList);
+        if (doReq) {
+          rank_publish(tile);
+          if (threadIdx.x == 0) {
+            if (total2) atomicAdd(&ctr->tilesWithExcess, 1u);
+            __threadfence();
+            atomicAdd(&ctr->tilesRanked, 1u);         // after the count above: tilesRanked == noTiles makes tilesWithExcess final
+          }
+        }
+        K2_STAMP(1);
+        // (A tile that still waits for other tiles' child marks leaves the mark bytes alone in this early pass: clearing a
+        // 16-byte group here could wipe a mark another tile is writing into it right now.)
+        if (doList) { decode(false, !deferList); if (!deferList) count_and_publish(tile); }
+        K2_STAMP(2);
+        if (doReq) {
+          serve(tile);
+          if (total2 != 0 && threadIdx.x == 0) {
+            __threadfence();                              // this tile's new child entries and their marks are visible device-wide ...
+            atomicAdd(&ctr->tilesExcessServed, 1u);       // ... before it counts as served
+          }
+        }
+        K2_STAMP(3);
+        K2_TILE_STAMP(4, tile);
+        if (!doList) continue;
+        if (deferList) {
+          // everything but this frame's new children is decoded already; wait until every tile with excess requests has
+          // served them (their number is final once all tiles have published their counts), then pick up the new marks
+          if (threadIdx.x == 0) {
+            while (*(volatile unsigned *)&ctr->tilesRanked < (unsigned)noTiles) { }
+            const unsigned need = *(volatile unsigned *)&ctr->tilesWithExcess;
+            while (*(volatile unsigned *)&ctr->tilesExcessServed < need) { }
+            __threadfence();
+          }
+          __syncthreads();
+          reload_marks();
+          decode(true, true);
+          count_and_publish(tile);
+        }
+        list_out(tile);
+      }
+    }
+  } else {
+    // Tiles from two tickets (draw_tile): pass 0 deals phase A of every tile and phase B of the ordered ones; pass 1, drawn only
+    // once pass 0's ticket has run out, deals phase B of the tiles that reach into the excess part, which wait for every tile's
+    // service first.
+    __shared__ int sTile;
+    const int firstDeferred = anyExcess ? numBuckets / AL_TILE : noTiles;
+    for (int pass = 0; pass < 2; ++pass) {
+      const bool doReq = pass == 0;
+      unsigned *const ticket = &ctr->ticket[doReq ? TK_SERVE : TK_SERVE_DEFERRED];
+      const int tile0 = doReq ? 0 : firstDeferred, passTiles = noTiles - tile0;
+      for (int k = draw_tile(ticket, passTiles, &sTile); k < passTiles; k = draw_tile(ticket, passTiles, &sTile)) {
+        const int tile = tile0 + k;
+        const bool doList = !doReq || tile < firstDeferred;
+        if (doReq) K2_TILE_STAMP(0, tile);
+        else {
+          // all of phase A is claimed (this ticket is drawn only after the first one ran out): wait for it, then read the marks
+          if (threadIdx.x == 0) {
+            while (*(volatile unsigned *)&ctr->tilesServed < (unsigned)noTiles) { }
+            __threadfence();
+          }
+          __syncthreads();
+        }
+        load_tile(tile, doReq, doList);
+        if (doReq) rank_publish(tile);
+        K2_STAMP(1);
+        if (doList) { decode(false, true); count_and_publish(tile); }
+        K2_STAMP(2);
+        if (doReq) {
+          serve(tile);
+          if (threadIdx.x == 0) {
+            __threadfence();                              // this tile's new entries and their marks are visible device-wide ...
+            atomicAdd(&ctr->tilesServed, 1u);             // ... before it counts as served
+          }
+          K2_STAMP(3);
+          K2_TILE_STAMP(4, tile);
+        }
+        if (doList) list_out(tile);
+      }
     }
   }
   // ---------------- the listed entries, dealt evenly over the grid ----------------
@@ -600,6 +665,9 @@ k_serve_list(const float *__restrict__ depth, b200_hash_entry *table, int numBuc
   __syncthreads();
   K2_STAMP(6);
   {
+    // ring position of item 0 (one 64-bit division per thread instead of one per listed entry). The ticketed form reads it from
+    // the snapshot the last tile published, not from its entry read: a CTA may have started after that tile moved ringHead on.
+    const long long ringBase = (TICKETED ? __ldcg(snapStart + slot) : ringStart) % ringCap;
     int nList = *(volatile int *)&ctr->noVisibleBlocks;
     if (nList > capacity) nList = capacity;
     for (int i0 = blockIdx.x * 32; i0 < nList; i0 += gridDim.x * 32) {
@@ -699,7 +767,10 @@ k_serve_list(const float *__restrict__ depth, b200_hash_entry *table, int numBuc
   if (threadIdx.x == 0) lastCta = (atomicAdd(&ctr->visCtasDone, 1u) == gridDim.x - 1);
   __syncthreads();
   if (!lastCta) return;
-  if (threadIdx.x == 0) { ctr->visCtasDone = 0; ctr->tilesRanked = 0; ctr->tilesWithExcess = 0; ctr->tilesExcessServed = 0; ctr->tilesListed = 0; ctr->anyExcessRequest = 0; }
+  if (threadIdx.x == 0) {
+    ctr->visCtasDone = 0; ctr->tilesRanked = 0; ctr->tilesWithExcess = 0; ctr->tilesExcessServed = 0; ctr->tilesServed = 0;
+    ctr->tilesListed = 0; ctr->anyExcessRequest = 0;
+  }
   __threadfence();
   if (!recs) return;
   // The last CTA knows the tile total. In the (pathological) case that it breaks MAX_RENDERING_BLOCKS it re-applies the
@@ -761,8 +832,10 @@ void launch_allocate(b200_engine *e, const SceneRef &s, const FrameGeom &g, cons
   const unsigned gen = ++e->scanGen;
   const int third = e->scanDescCap / 3;
   trace_begin(e, st, "k_serve_list");
-  // chained in every caller: the list kernel always directly follows the marking kernel
-  launch_chained(true, k_serve_list, persistent_grid(e, 2, noTiles), 256, 0, st, depth, s.hash, s.numBuckets, s.noTotal, s.visType,
+  // chained in every caller: the list kernel always directly follows the marking kernel. The ticketed form whenever another
+  // engine shares the device (its kernels may hold SMs this grid needs) or the grid is scaled beyond what the GPU holds.
+  const bool ticketed = e->gridScale > 1 || device_shared(e);
+  launch_chained(true, ticketed ? k_serve_list<true> : k_serve_list<false>, ticketed ? ticket_grid(e, 2, noTiles) : persistent_grid(e, 2, noTiles), 256, 0, st, depth, s.hash, s.numBuckets, s.noTotal, s.visType,
                  e->d_reqKey, e->d_reqBits, e->d_req2Bits, e->d_markBytes, s.allocationList, s.excessList, e->d_ctr, g, frameIdx,
                  onlyVisible ? 1 : 0, e->d_scanDesc, e->d_scanDesc + third, e->d_scanDesc + 2 * third, gen, s.visiblePos, e->d_visiblePtr,
                  s.numBlocks, e->d_ring, e->ringCap, e->d_snapStart, e->d_snapCount, snapSlot,

@@ -35,7 +35,7 @@ static_assert(sizeof(b200_checkpoint_header) == B200_CHECKPOINT_HEADER_BYTES, "c
 struct CheckpointScratch {
   unsigned *d_blkIds, *d_entIdx, *d_visIdx;   // classification: ascending indices of the blocks / entries / bytes kept
   unsigned long long *d_desc;                 // chained-scan descriptors: block tiles, entry tiles, visibility tiles
-  int tilesB, tilesE, classifyGrid;
+  int tilesB, tilesE, classifyGrid, classifyPerSm;   // classifyPerSm: resident classification CTAs per SM (occupancy)
   long long *d_counts, *h_counts;             // noBlocks, noEntries, noVisBytes (device, pinned mirror)
   int *d_qCount; long long *d_qCum, *d_qStart;   // save: the queue table (SNAP_SLOTS entries, cumulative counts + 1)
   int *h_snapCount; long long *h_snapStart;   // pinned copies of the engine's snapshot slots
@@ -51,14 +51,16 @@ struct CheckpointScratch {
 // ---- kernels ---------------------------------------------------------------------------------------------------------
 
 // Tiles [0, tilesB) test voxel blocks, [tilesB, tilesB + tilesE) hash entries and visibility bytes; each kind is compacted
-// through its own descriptor chain. Persistent grid: every tile's predecessors are owned by resident CTAs (common.cuh).
+// through its own descriptor chain. Tiles come from draw_tile, so every tile's predecessors are owned by running CTAs (common.cuh).
 __global__ void __launch_bounds__(256)
 k_ck_classify(const uint4 *voxels, int numBlocks, const int *hash, const uint8_t *visType, int noTotal, int tilesB, int tilesE,
-              unsigned long long *desc, unsigned gen, unsigned *blkIds, unsigned *entIdx, unsigned *visIdx, long long *counts) {
+              unsigned long long *desc, unsigned gen, unsigned *blkIds, unsigned *entIdx, unsigned *visIdx, long long *counts,
+              unsigned *ticket) {
   __shared__ unsigned sm[33];
   __shared__ unsigned base[2];
+  __shared__ int sTile;
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  for (int t = blockIdx.x; t < tilesB + tilesE; t += gridDim.x) {
+  for (int t = draw_tile(ticket, tilesB + tilesE, &sTile); t < tilesB + tilesE; t = draw_tile(ticket, tilesB + tilesE, &sTile)) {
     if (t < tilesB) {
       const int first = t * CK_TILE_BLOCKS + warp * 32;
       unsigned mask = 0;                      // bit i: block first + i differs from a reset block
@@ -269,7 +271,8 @@ static b200_status ck_ensure(b200_engine *e, size_t smallBytes) {
     CK(cudaStreamCreateWithFlags(&c->copyStream, cudaStreamNonBlocking));
     int perSm = 0;
     CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&perSm, k_ck_classify, 256, 0));
-    c->classifyGrid = persistent_grid(e, perSm > 0 ? perSm : 1, (long long)c->tilesB + c->tilesE);
+    c->classifyPerSm = perSm > 0 ? perSm : 1;
+    c->classifyGrid = persistent_grid(e, c->classifyPerSm, (long long)c->tilesB + c->tilesE);
   }
   CheckpointScratch *c = e->ck;
   if (smallBytes > c->smallCap) {
@@ -334,9 +337,10 @@ b200_status b200_checkpoint_save(b200_engine *e, b200_scene *s, b200_render_stat
   if (!h_out || !(c->valid && c->launches == e->launches && c->voxels == s->d_voxels && c->hash == s->d_hash &&
                   c->visType == rs->d_entriesVisibleType)) {
     TRACED(e, e->stream, "k_ck_classify",
-           k_ck_classify<<<c->classifyGrid, 256, 0, e->stream>>>((const uint4 *)s->d_voxels, s->numBlocks, (const int *)s->d_hash,
+           k_ck_classify<<<ticket_grid(e, c->classifyPerSm, (long long)c->tilesB + c->tilesE), 256, 0, e->stream>>>((const uint4 *)s->d_voxels, s->numBlocks, (const int *)s->d_hash,
                                                                  rs->d_entriesVisibleType, e->noTotal, c->tilesB, c->tilesE, c->d_desc,
-                                                                 ++e->scanGen, c->d_blkIds, c->d_entIdx, c->d_visIdx, c->d_counts));
+                                                                 ++e->scanGen, c->d_blkIds, c->d_entIdx, c->d_visIdx, c->d_counts,
+                                                                 &e->d_ctr->ticket[TK_CK_CLASSIFY]));
     e->launches++;
     CK(cudaMemcpyAsync(c->h_counts, c->d_counts, 3 * sizeof(long long), cudaMemcpyDeviceToHost, e->stream));
     CK(cudaStreamSynchronize(e->stream));

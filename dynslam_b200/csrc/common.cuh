@@ -101,6 +101,9 @@ DEV int find_block(const b200_hash_entry *table, int numBuckets, int x, int y, i
 }
 
 // ---- device-resident counters (mirrored to pinned host memory by the engine) ----------------
+// tile tickets of the kernels whose CTAs wait on one another (draw_tile), one counter each
+enum { TK_SERVE, TK_SERVE_DEFERRED, TK_FREEVIEW, TK_DECAY_RANK, TK_MESH_LIST, TK_MESH_BLOCKS, TK_CK_CLASSIFY, TK_SWAP_LIST,
+       TK_FWD_MISSING, TK_POINT_CLOUD, TK_COUNT };
 struct DevCounters {
   int lastFreeBlockId;
   int lastFreeExcessListId;
@@ -119,10 +122,11 @@ struct DevCounters {
   unsigned noRenderingBlocks;
   unsigned visCtasDone;    // k_serve_list: CTAs that have finished (the last one applies the rendering-block cap if needed)
   unsigned depthCtasDone;  // k_expected_depths: the same for the stand-alone CreateExpectedDepths
-  unsigned listTicket;     // k_freeview_list: next table tile to hand out (reset by the launch's last draw)
-  unsigned tilesRanked;    // k_serve_list: tiles that have published their request counts
-  unsigned tilesListed;    // ... that have written their part of the visible list (the per-entry phase starts when all have)
+  unsigned ticket[TK_COUNT];   // next tile to hand out, per kernel (draw_tile; reset by each launch's last draw)
+  unsigned tilesRanked;    // k_serve_list, CTA-owned tiles: tiles that have published their request counts
   unsigned tilesWithExcess, tilesExcessServed;   // ... of which have excess-list requests / have served them (excess-part tiles list only after all have)
+  unsigned tilesServed;    // k_serve_list, ticketed tiles: tiles that have ranked and served their requests
+  unsigned tilesListed;    // both forms: tiles that have written their part of the visible list (the per-entry phase starts when all have)
   int anyExcessRequest;    // set by the marking kernel when it files an excess-list request; cleared by k_serve_list's last CTA
   int noNeededEntries;     // swapping
   unsigned noTotalPoints;
@@ -134,9 +138,27 @@ struct DevCounters {
   int integDone;           // k_integrate_v3: CTAs that have stopped claiming; the last one zeroes both for the next launch
 };
 
+// ---- tile hand-out for kernels whose CTAs wait on one another --------------------------------
+// A CTA that waits on another CTA (a chained scan's look-back, a device-wide counter) waits only on work that a running CTA has
+// already claimed. Tiles are therefore drawn from a ticket counter, never owned by blockIdx: tile t is claimed only after tiles
+// 0 .. t-1 have been, each by a CTA that is running and that waits, in turn, only on lower tiles, so the grid need not be
+// resident all at once (other engines' kernels on the same GPU, or a grid larger than the GPU holds: b200_diag_set_grid_scale).
+// Every CTA draws until it gets a ticket past the last tile, so each CTA draws exactly one such ticket and draw
+// noTiles + gridDim.x - 1 is the launch's last: the CTA that makes it resets the counter for the next launch. Called by every
+// thread of the CTA, after the kernel's pdl_wait(); all CTAs pass the same noTiles. Returns the tile (>= noTiles: none left).
+DEV int draw_tile(unsigned *ticket, int noTiles, int *slot /* __shared__ */) {
+  __syncthreads();                     // every thread has read the previous draw
+  if (threadIdx.x == 0) {
+    const unsigned t = atomicAdd(ticket, 1u);
+    if (t == (unsigned)noTiles + gridDim.x - 1) *ticket = 0;
+    *slot = (int)t;
+  }
+  __syncthreads();
+  return *slot;
+}
+
 // ---- chained-scan (decoupled look-back) for ordered compaction --------------------------------
-// Persistent grids only (gridDim.x <= co-resident CTAs) so that every predecessor tile is owned by
-// a resident CTA: tile t is processed by CTA (t % gridDim.x) in round t / gridDim.x.
+// Tiles come from draw_tile, so every predecessor tile is owned by a CTA that is running.
 // Descriptor: [63:34] generation (30 bit) | [33:32] status (1 = aggregate, 2 = inclusive prefix) |
 // [31:0] value. A fresh generation per launch makes resets unnecessary.
 DEV unsigned long long scan_pack(unsigned gen, unsigned status, unsigned value) {

@@ -78,10 +78,12 @@ k_decay_rank(const int *itemPtr, const unsigned long long *delTag, unsigned gen,
              unsigned long long *scanDesc, unsigned scanGen) {
   __shared__ unsigned sm[33];
   __shared__ unsigned tileBase;
+  __shared__ int sTile;
   const int n = ctr->decayItems;
   const int lastFree = ctr->lastFreeBlockId;
   const int noTiles = (n + DEC_TILE - 1) / DEC_TILE;
-  for (int tile = blockIdx.x; tile < noTiles; tile += gridDim.x) {
+  unsigned *ticket = &ctr->ticket[TK_DECAY_RANK];
+  for (int tile = draw_tile(ticket, noTiles, &sTile); tile < noTiles; tile = draw_tile(ticket, noTiles, &sTile)) {
     const int first = tile * DEC_TILE + threadIdx.x * 4;
     unsigned mask = 0;
     int ptrs[4];
@@ -108,7 +110,6 @@ k_decay_rank(const int *itemPtr, const unsigned long long *delTag, unsigned gen,
       delList[r] = first + k;
       r++;
     }
-    __syncthreads();
   }
   if (noTiles == 0 && blockIdx.x == 0 && threadIdx.x == 0) ctr->decayDeleted = 0;
 }
@@ -360,7 +361,7 @@ void launch_decay_full(b200_engine *e, const SceneRef &s, int minAge, int maxWei
   k_decay_sweep<1><<<sweep_grid(e, s), 256, 0, st>>>(d);
   trace_end(e, st);
   const int noTiles = (s.numBlocks + DEC_TILE - 1) / DEC_TILE;
-  k_decay_rank<<<persistent_grid(e, 4, noTiles), 256, 0, st>>>(e->d_itemPtr, e->d_delTag, gen, s.allocationList, e->d_delList,
+  k_decay_rank<<<ticket_grid(e, 4, noTiles), 256, 0, st>>>(e->d_itemPtr, e->d_delTag, gen, s.allocationList, e->d_delList,
                                                                e->d_ctr, e->d_scanDesc, ++e->scanGen);
   k_decay_elect<1><<<e->smCount, 128, 0, st>>>(s.hash, s.numBuckets, e->d_ring, e->ringCap, e->d_snapStart, 0, e->d_allocatedPos,
                                               e->d_delList, e->d_delTag, gen, e->d_isLeader, e->d_ctr);

@@ -9,6 +9,7 @@
 // shim calls, which must return with host-visible counters valid) do exactly one asynchronous
 // upload, the launches, one asynchronous download and one stream synchronise; the fused
 // b200_process_frame_async path does none of that until b200_sync().
+#include <atomic>
 #include "engine.h"
 #include "../../include/b200fusion_diag.h"
 
@@ -95,6 +96,15 @@ b200_status download_sync(b200_engine *e, b200_scene *s, b200_render_state *rs) 
   return B200_OK;
 }
 
+// Live engines per device. k_serve_list owns its tiles by blockIdx while an engine is alone on its device (the faster form, which
+// needs the whole grid resident) and draws them by ticket once another engine shares the device (device_shared).
+#define B200_MAX_DEVICES 64
+static std::atomic<int> g_liveEngines[B200_MAX_DEVICES];
+
+bool device_shared(const b200_engine *e) {
+  return e->device < 0 || e->device >= B200_MAX_DEVICES || g_liveEngines[e->device].load(std::memory_order_relaxed) > 1;
+}
+
 extern "C" {
 
 static b200_status engine_create_body(const b200_engine_config *cfg, b200_engine *e);
@@ -113,12 +123,23 @@ b200_status b200_engine_create(const b200_engine_config *cfg, b200_engine **out)
     b200_engine_destroy(e);
     return st;
   }
+  if (e->device >= 0 && e->device < B200_MAX_DEVICES) {
+    e->registered = true;
+    // The engines already on the device may have grids of the blockIdx form in flight, which must not run beside this engine's
+    // kernels: wait for the device once, here, after which every engine on it enqueues the ticketed form.
+    if (g_liveEngines[e->device].fetch_add(1) > 0 && cudaDeviceSynchronize() != cudaSuccess) {
+      snprintf(g_createErr, sizeof(g_createErr), "cudaDeviceSynchronize failed: %s", cudaGetErrorString(cudaGetLastError()));
+      b200_engine_destroy(e);
+      return B200_ERR_CUDA;
+    }
+  }
   *out = e;
   return B200_OK;
 }
 
 static b200_status engine_create_body(const b200_engine_config *cfg, b200_engine *e) {
   e->maxRenderingBlocks = B200_MAX_RENDERING_BLOCKS;
+  e->gridScale = 1;
   e->device = cfg->device;
   e->numBlocks = cfg->numBlocks; e->numBuckets = cfg->numBuckets; e->excessSize = cfg->excessSize;
   e->noTotal = cfg->numBuckets + cfg->excessSize; e->img_w = cfg->img_w; e->img_h = cfg->img_h;
@@ -212,6 +233,7 @@ void b200_engine_destroy(b200_engine *e) {
   if (!e) return;
   cudaSetDevice(e->device);
   if (e->stream) cudaStreamSynchronize(e->stream);
+  if (e->registered) g_liveEngines[e->device].fetch_sub(1);
   cudaFree(e->d_ctr); cudaFreeHost(e->h_ctr); cudaFree(e->d_reqKey); cudaFree(e->d_reqBits); cudaFree(e->d_markBytes); cudaFree(e->d_dbg); cudaFree(e->d_meshDesc); cudaFree(e->d_evalCounters); cudaFreeHost(e->h_evalCounters); cudaFree(e->d_scanDesc);
   cudaFree(e->d_ring); cudaFree(e->d_snapCount); cudaFree(e->d_snapStart); cudaFree(e->d_delTag); cudaFree(e->d_itemPtr); cudaFree(e->d_resetPtr); cudaFree(e->d_visiblePtr);
   cudaFree(e->d_viewScratch); cudaFree(e->d_delList); cudaFree(e->d_candList); cudaFree(e->d_isLeader); cudaFree(e->d_allocatedPos); cudaFree(e->d_tileCounts); cudaFree(e->d_blockRecs);
@@ -278,6 +300,8 @@ int b200_get_trace(b200_engine *e, char *out, int cap) {
 }
 
 void b200_diag_set_max_rendering_blocks(b200_engine *e, int n) { e->maxRenderingBlocks = n > 0 ? n : B200_MAX_RENDERING_BLOCKS; }
+
+void b200_diag_set_grid_scale(b200_engine *e, int k) { e->gridScale = k > 1 ? (k < 64 ? k : 64) : 1; }
 
 void b200_diag_last_integrate(const b200_engine *e, int *kernel, int *grid) {
   if (kernel) *kernel = e->lastIntegrateKernel;
@@ -414,7 +438,7 @@ b200_status b200_find_visible_blocks(b200_engine *e, const b200_scene *s, b200_r
   st = upload(e, s, rs); if (st) return st;
   if (e->ptrListFor == (const void *)rs->d_visibleBlockPositions) e->ptrListFor = nullptr;   // list rebuilt without ptrs
   launch_find_visible(e, scene_ref(s, rs), to_mat(cam->M), cam->proj, rs->img_w, rs->img_h, s->voxelSize, &e->d_ctr->noVisibleBlocks,
-                      &e->d_ctr->listTicket, e->d_scanDesc, ++e->scanGen);
+                      &e->d_ctr->ticket[TK_FREEVIEW], e->d_scanDesc, ++e->scanGen);
   return download_sync(e, nullptr, rs);
 }
 

@@ -82,6 +82,8 @@ struct b200_engine {
   cudaEvent_t evH2D[2], evCompute[2], evD2H[2];
   bool slotBusy[2]; size_t stagePixels;
   int maxRenderingBlocks;                           // MAX_RENDERING_BLOCKS; b200_diag_set_max_rendering_blocks lowers it (tests)
+  int gridScale;                                    // ticket_grid's factor, 1; b200_diag_set_grid_scale raises it (tests)
+  bool registered;                                  // counted among the device's live engines (device_shared, engine.cu)
   int useGraph; bool graphWarm; cudaGraphExec_t frameGraph;
   cudaEvent_t evMid; bool midValid;                 // "allocation + integration of the last frame are done" (pipelined uploads wait for it)         // B200_GRAPH=1: the fused frame is captured and replayed as a CUDA graph
   float *d_viewScratch; size_t viewScratchPixels;   // plays view->depth inside UpdateView (view.cu)
@@ -272,3 +274,11 @@ static inline int persistent_grid(const b200_engine *e, int ctasPerSm, long long
   if (workItems < g) g = workItems;
   return (int)(g < 1 ? 1 : g);
 }
+// grid of a kernel that hands out its tiles with draw_tile: persistent_grid, or with b200_diag_set_grid_scale's factor k > 1,
+// k times the whole GPU's worth of CTAs whatever the number of tiles (ctasPerSm >= 1 and k >= 8 are at least the 2048 threads an
+// SM holds for CTAs of 256 threads or more, so most CTAs start only after others have retired)
+static inline int ticket_grid(const b200_engine *e, int ctasPerSm, long long workItems) {
+  return e->gridScale > 1 ? e->smCount * ctasPerSm * e->gridScale : persistent_grid(e, ctasPerSm, workItems);
+}
+// another engine is live on this engine's device (engine.cu counts them); k_serve_list then hands out its tiles by ticket
+bool device_shared(const b200_engine *e);

@@ -85,11 +85,13 @@ DEV V3 colour_at(const b200_voxel *__restrict__ voxels, const b200_hash_entry *_
 #define ML_EPT 16
 #define ML_TILE (256 * ML_EPT)
 __global__ void __launch_bounds__(256)
-k_mesh_list(const b200_hash_entry *__restrict__ table, int noTotal, int *list, int capacity, unsigned *count, unsigned long long *scanDesc, unsigned gen) {
+k_mesh_list(const b200_hash_entry *__restrict__ table, int noTotal, int *list, int capacity, unsigned *count, unsigned long long *scanDesc, unsigned gen,
+            unsigned *ticket) {
   __shared__ unsigned sm[33];
   __shared__ unsigned tileBase;
+  __shared__ int sTile;
   const int noTiles = (noTotal + ML_TILE - 1) / ML_TILE;
-  for (int tile = blockIdx.x; tile < noTiles; tile += gridDim.x) {
+  for (int tile = draw_tile(ticket, noTiles, &sTile); tile < noTiles; tile = draw_tile(ticket, noTiles, &sTile)) {
     const int first = tile * ML_TILE + threadIdx.x * ML_EPT;
     unsigned mask = 0;
 #pragma unroll
@@ -109,7 +111,6 @@ k_mesh_list(const b200_hash_entry *__restrict__ table, int noTotal, int *list, i
       if ((int)o < capacity) list[o] = first + k;
       o++;
     }
-    __syncthreads();
   }
 }
 
@@ -117,14 +118,15 @@ k_mesh_list(const b200_hash_entry *__restrict__ table, int noTotal, int *list, i
 __global__ void __launch_bounds__(512)
 k_mesh_blocks(const b200_voxel *__restrict__ voxels, const b200_hash_entry *__restrict__ table, int nb, const int *__restrict__ list,
               const unsigned *__restrict__ listCount, int capacity, float factor, b200_triangle *triangles, unsigned noMaxTriangles,
-              unsigned *noTotalTriangles, unsigned long long *scanDesc, unsigned gen) {
+              unsigned *noTotalTriangles, unsigned long long *scanDesc, unsigned gen, unsigned *ticket) {
   __shared__ unsigned sm[33];
   __shared__ unsigned tileBase;
+  __shared__ int sTile;
   unsigned n = *listCount;
   if (n > (unsigned)capacity) n = (unsigned)capacity;
   if (n == 0) { if (blockIdx.x == 0 && threadIdx.x == 0) *noTotalTriangles = 0; return; }
   const int x = threadIdx.x & 7, y = (threadIdx.x >> 3) & 7, z = threadIdx.x >> 6;
-  for (unsigned tile = blockIdx.x; tile < n; tile += gridDim.x) {
+  for (unsigned tile = draw_tile(ticket, (int)n, &sTile); tile < n; tile = draw_tile(ticket, (int)n, &sTile)) {
     const Entry en = load_entry(table, list[tile]);
     const int gx = en.x * BS + x, gy = en.y * BS + y, gz = en.z * BS + z;
     float sdf[8];
@@ -168,7 +170,6 @@ k_mesh_blocks(const b200_voxel *__restrict__ voxels, const b200_hash_entry *__re
         triangles[id] = T;
       }
     }
-    __syncthreads();
   }
 }
 
@@ -181,8 +182,10 @@ void launch_mesh_scene(b200_engine *e, const SceneRef &s, float voxelSize, b200_
     cudaMemsetAsync(e->d_meshDesc, 0, sizeof(unsigned long long) * (size_t)(e->numBlocks + 1), e->stream);
   }
   const int listTiles = (s.noTotal + ML_TILE - 1) / ML_TILE;
-  k_mesh_list<<<persistent_grid(e, 4, listTiles), 256, 0, e->stream>>>(s.hash, s.noTotal, e->d_delList, s.numBlocks, count, e->d_scanDesc, ++e->scanGen);
-  k_mesh_blocks<<<persistent_grid(e, 2, s.numBlocks), 512, 0, e->stream>>>(s.voxels, s.hash, s.numBuckets, e->d_delList, count, s.numBlocks, voxelSize,
-                                                                           triangles, noMaxTriangles, total, e->d_meshDesc, ++e->scanGen);
+  k_mesh_list<<<ticket_grid(e, 4, listTiles), 256, 0, e->stream>>>(s.hash, s.noTotal, e->d_delList, s.numBlocks, count, e->d_scanDesc, ++e->scanGen,
+                                                                    &e->d_ctr->ticket[TK_MESH_LIST]);
+  k_mesh_blocks<<<ticket_grid(e, 2, s.numBlocks), 512, 0, e->stream>>>(s.voxels, s.hash, s.numBuckets, e->d_delList, count, s.numBlocks, voxelSize,
+                                                                       triangles, noMaxTriangles, total, e->d_meshDesc, ++e->scanGen,
+                                                                       &e->d_ctr->ticket[TK_MESH_BLOCKS]);
   e->launches += 2;
 }

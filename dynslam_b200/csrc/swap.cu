@@ -17,8 +17,10 @@ k_swap_list(const uint8_t *__restrict__ swapStates, const b200_hash_entry *__res
             int noTotal, int *needed, DevCounters *ctr, unsigned long long *scanDesc, unsigned gen) {
   __shared__ unsigned sm[33];
   __shared__ unsigned tileBase;
+  __shared__ int sTile;
   const int noTiles = (noTotal + SWAP_TILE - 1) / SWAP_TILE;
-  for (int tile = blockIdx.x; tile < noTiles; tile += gridDim.x) {
+  unsigned *ticket = &ctr->ticket[TK_SWAP_LIST];
+  for (int tile = draw_tile(ticket, noTiles, &sTile); tile < noTiles; tile = draw_tile(ticket, noTiles, &sTile)) {
     const int first = tile * SWAP_TILE + threadIdx.x * 16;
     unsigned mask = 0;
     for (int k = 0; k < 16; ++k) {
@@ -48,19 +50,18 @@ k_swap_list(const uint8_t *__restrict__ swapStates, const b200_hash_entry *__res
       if (o < B200_TRANSFER_BLOCK_NUM) needed[o] = first + k;
       o++;
     }
-    __syncthreads();
   }
 }
 
 void launch_swap_list_in(b200_engine *e, const SceneRef &s, int *needed) {
   const int noTiles = (s.noTotal + SWAP_TILE - 1) / SWAP_TILE;
-  k_swap_list<0><<<persistent_grid(e, 4, noTiles), 256, 0, e->stream>>>(s.swapStates, s.hash, s.visType, s.noTotal, needed, e->d_ctr,
+  k_swap_list<0><<<ticket_grid(e, 4, noTiles), 256, 0, e->stream>>>(s.swapStates, s.hash, s.visType, s.noTotal, needed, e->d_ctr,
                                                                        e->d_scanDesc, ++e->scanGen);
   e->launches++;
 }
 void launch_swap_list_out(b200_engine *e, const SceneRef &s, int *needed) {
   const int noTiles = (s.noTotal + SWAP_TILE - 1) / SWAP_TILE;
-  k_swap_list<1><<<persistent_grid(e, 4, noTiles), 256, 0, e->stream>>>(s.swapStates, s.hash, s.visType, s.noTotal, needed, e->d_ctr,
+  k_swap_list<1><<<ticket_grid(e, 4, noTiles), 256, 0, e->stream>>>(s.swapStates, s.hash, s.visType, s.noTotal, needed, e->d_ctr,
                                                                        e->d_scanDesc, ++e->scanGen);
   e->launches++;
 }

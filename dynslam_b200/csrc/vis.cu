@@ -23,10 +23,7 @@
 // ------------------------------------------------------------------------------------------------
 // FindVisibleBlocks: every entry with ptr >= 0 that passes the frustum test, ascending entry order; the visibility bytes are
 // not touched. *count receives the number found, not capped by the list's capacity (the reference's count is not either).
-// Tiles are handed out through a ticket, not by blockIdx: a tile then only ever waits for tiles whose CTAs are already
-// running, so the chained scan's look-back cannot stall when the grid is not co-resident (two engines' sweeps sharing the
-// GPU). Every CTA draws exactly one ticket past the last tile, so ticket noTiles + gridDim.x - 1 is the launch's last draw and
-// the CTA that draws it resets the ticket for the next launch.
+// Tiles come from the caller's ticket (draw_tile, common.cuh).
 __global__ void __launch_bounds__(256, 4)
 k_freeview_list(const b200_hash_entry *__restrict__ table, int noTotal, b200_vec3i *visiblePos, int capacity, int *count,
                 unsigned *ticket, unsigned long long *scanDesc, unsigned gen, Mat4 M, float p0, float p1, float p2, float p3,
@@ -36,15 +33,7 @@ k_freeview_list(const b200_hash_entry *__restrict__ table, int noTotal, b200_vec
   __shared__ int sTile;
   const float proj[4] = {p0, p1, p2, p3};
   const int noTiles = (noTotal + FV_TILE - 1) / FV_TILE;
-  for (;;) {
-    if (threadIdx.x == 0) {
-      const unsigned t = atomicAdd(ticket, 1u);
-      if (t == (unsigned)noTiles + gridDim.x - 1) *ticket = 0;
-      sTile = (int)t;
-    }
-    __syncthreads();
-    const int tile = sTile;
-    if (tile >= noTiles) break;
+  for (int tile = draw_tile(ticket, noTiles, &sTile); tile < noTiles; tile = draw_tile(ticket, noTiles, &sTile)) {
     // strided assignment inside the tile keeps the 20-byte entry reads of a warp adjacent
     unsigned mask = 0;
     for (int k = 0; k < FV_EPT; ++k) {
@@ -76,7 +65,6 @@ k_freeview_list(const b200_hash_entry *__restrict__ table, int noTotal, b200_vec
       const unsigned o = tileBase + offs[k];
       if ((int)o < capacity) { b200_vec3i p; p.x = en.x; p.y = en.y; p.z = en.z; visiblePos[o] = p; }
     }
-    __syncthreads();
   }
 }
 
@@ -84,7 +72,7 @@ void launch_find_visible(b200_engine *e, const SceneRef &s, const Mat4 &M, const
                          int *count, unsigned *ticket, unsigned long long *scanDesc, unsigned gen) {
   const int noTiles = (s.noTotal + FV_TILE - 1) / FV_TILE;
   trace_begin(e, e->stream, "k_freeview_list");
-  k_freeview_list<<<persistent_grid(e, 4, noTiles), 256, 0, e->stream>>>(s.hash, s.noTotal, s.visiblePos, s.numBlocks, count, ticket,
+  k_freeview_list<<<ticket_grid(e, 4, noTiles), 256, 0, e->stream>>>(s.hash, s.noTotal, s.visiblePos, s.numBlocks, count, ticket,
                                                                         scanDesc, gen, M, proj[0], proj[1], proj[2], proj[3], voxelSize,
                                                                         w, h);
   trace_end(e, e->stream);
@@ -467,8 +455,10 @@ k_fwd_gather_missing(const float4 *__restrict__ rays, const int *__restrict__ wi
                      unsigned gen) {
   __shared__ unsigned sm[33];
   __shared__ unsigned tileBase;
+  __shared__ int sTile;
   const int n = w * h, noTiles = (n + FWD_TILE - 1) / FWD_TILE;
-  for (int tile = blockIdx.x; tile < noTiles; tile += gridDim.x) {
+  unsigned *ticket = &ctr->ticket[TK_FWD_MISSING];
+  for (int tile = draw_tile(ticket, noTiles, &sTile); tile < noTiles; tile = draw_tile(ticket, noTiles, &sTile)) {
     unsigned mask = 0;
     const int first = tile * FWD_TILE + threadIdx.x * 4;
 #pragma unroll
@@ -494,7 +484,6 @@ k_fwd_gather_missing(const float4 *__restrict__ rays, const int *__restrict__ wi
     unsigned o = tileBase + local;
 #pragma unroll
     for (int k = 0; k < 4; ++k) if (mask & (1u << k)) missing[o++] = first + k;
-    __syncthreads();
   }
 }
 
@@ -521,7 +510,7 @@ void launch_forward_render(b200_engine *e, const SceneRef &s, const FrameGeom &g
   k_fwd_splat<<<(n + 255) / 256, 256, 0, st>>>((const float4 *)rays, g.w, g.h, g.M_d, g.proj_d[0], g.proj_d[1], g.proj_d[2], g.proj_d[3],
                                               g.voxelSize, winner);
   const int noTiles = (n + FWD_TILE - 1) / FWD_TILE;
-  k_fwd_gather_missing<<<persistent_grid(e, 4, noTiles), 256, 0, st>>>((const float4 *)rays, winner, (float4 *)fwd, depth,
+  k_fwd_gather_missing<<<ticket_grid(e, 4, noTiles), 256, 0, st>>>((const float4 *)rays, winner, (float4 *)fwd, depth,
                                                                       (const float2 *)minmax, g.w, g.h, missing, e->d_ctr, e->d_scanDesc,
                                                                       ++e->scanGen);
   k_fwd_raycast_missing<<<e->smCount * 4, 128, 0, st>>>((float4 *)fwd, missing, e->d_ctr, s.voxels, s.hash, s.numBuckets, g.w, g.invM_d,
@@ -545,8 +534,10 @@ k_point_cloud(const float4 *__restrict__ rays, const b200_voxel *__restrict__ vo
               DevCounters *ctr, unsigned long long *scanDesc, unsigned gen) {
   __shared__ unsigned sm[33];
   __shared__ unsigned tileBase;
+  __shared__ int sTile;
   const int n = w * h, noTiles = (n + 255) / 256;
-  for (int tile = blockIdx.x; tile < noTiles; tile += gridDim.x) {
+  unsigned *ticket = &ctr->ticket[TK_POINT_CLOUD];
+  for (int tile = draw_tile(ticket, noTiles, &sTile); tile < noTiles; tile = draw_tile(ticket, noTiles, &sTile)) {
     const int locId = tile * 256 + threadIdx.x;
     bool found = false; float4 pr = make_float4(0, 0, 0, 0);
     if (locId < n) {
@@ -574,14 +565,13 @@ k_point_cloud(const float4 *__restrict__ rays, const b200_voxel *__restrict__ vo
       colours[o] = tmp;
       locations[o] = make_float4(pr.x * voxelSize, pr.y * voxelSize, pr.z * voxelSize, 1.0f);
     }
-    __syncthreads();
   }
 }
 
 void launch_point_cloud(b200_engine *e, const SceneRef &s, const Mat4 &invM, int w, int h, float voxelSize, int skipPoints,
                         const b200_vec4f *rays, b200_vec4u *outImg, b200_vec4f *locations, b200_vec4f *colours) {
   const int noTiles = (w * h + 255) / 256;
-  k_point_cloud<<<persistent_grid(e, 2, noTiles), 256, 0, e->stream>>>((const float4 *)rays, s.voxels, s.hash, s.numBuckets, w, h,
+  k_point_cloud<<<ticket_grid(e, 2, noTiles), 256, 0, e->stream>>>((const float4 *)rays, s.voxels, s.hash, s.numBuckets, w, h,
                                                                       -invM.m[8], -invM.m[9], -invM.m[10], voxelSize, skipPoints,
                                                                       (uchar4 *)outImg, (float4 *)locations, (float4 *)colours, e->d_ctr,
                                                                       e->d_scanDesc, ++e->scanGen);

@@ -221,6 +221,11 @@ class Engine:
         """test hook (include/b200fusion_diag.h): lower MAX_RENDERING_BLOCKS to reach the cap rule with small scenes"""
         self.lib.b200_diag_set_max_rendering_blocks(self.h, int(n))
 
+    def set_grid_scale(self, k):
+        """test hook (include/b200fusion_diag.h): launch the kernels whose CTAs wait on one another on k times their grid,
+        more CTAs than the GPU holds at once; k <= 1 restores the default"""
+        self.lib.b200_diag_set_grid_scale(self.h, int(k))
+
     def last_integrate(self):
         """test hook (include/b200fusion_diag.h): (kernel, grid) of the last integrate launch; kernel 0 LDG, 1 TMA, 2 V3, 3 V4 with
         two voxels per lane, 4 V4 with four, + 8 in tolerance mode"""

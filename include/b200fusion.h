@@ -140,6 +140,19 @@ typedef enum {                 /* IITMVisualisationEngine::RenderImageType, Vis.
 
 /* ---- engine handle ---------------------------------------------------------------------- */
 
+/* One engine per volume. Engines on one device may have any of their calls in flight at the same time, each on its own
+   stream: no kernel of the library waits on a CTA that has not started, so a volume's work completes whatever other engines'
+   kernels hold the GPU, and its results are byte for byte those of the same calls run alone. The order between volumes is the
+   caller's, set with b200_engine_wait_engine. (An engine alone on its device runs a faster form of the allocation's list pass
+   that needs its whole grid resident; creating a second engine on the device waits once for the device, b200_engine_create,
+   after which every engine there runs the form that does not. Create engines from the thread that enqueues their work.)
+   DynSLAM's frame (static map + K car volumes, one GPU), with no host wait:
+     1. b200_process_silhouettes_async on the static engine's stream (cuts the car frames out of the input);
+     2. every car engine: b200_engine_wait_engine(car, static), then b200_process_frame_async of its volume;
+     3. b200_process_frame_async of the static map;
+     4. b200_engine_wait_engine(static, car) for every car, then b200_composite_instances on the static engine.
+   Stand-alone calls (b200_decay with forceAllVoxels for Reap, b200_mesh_scene, b200_checkpoint_save) on one engine may run
+   while the other engines' frames are in flight; they wait for their own engine's stream only. */
 typedef struct b200_engine b200_engine;
 
 typedef struct {
@@ -319,7 +332,8 @@ b200_status b200_render_view_wait(b200_engine *e, int slot);   /* the host waits
 /* e's stream waits, on the device, for everything enqueued so far on producer's stream (an event record and a
    cudaStreamWaitEvent; the host does not wait). This is what lets one engine composite layers other engines rendered
    (b200_composite_instances, b200_composite_depth) with no host synchronisation between the renders and the composite.
-   Engines on the same device or on peers. */
+   Engines on the same device or on peers. It is the only ordering between engines: calls of engines on one device that do
+   not wait for each other run concurrently (see the engine handle above for the frame sequence of one GPU). */
 b200_status b200_engine_wait_engine(b200_engine *e, b200_engine *producer);
 
 /* ---- view builder (SURVEY 8(f) rank 1): the step immediately before fusion ------------------------

@@ -45,6 +45,14 @@ b200_status b200_selftest_divide(b200_engine *e, uint64_t pairs, uint64_t seed, 
    (Vis_CUDA.cu:609) with small scenes. n <= 0 restores the reference's constant. */
 void b200_diag_set_max_rendering_blocks(b200_engine *e, int n);
 
+/* Launch this engine's kernels whose CTAs wait on one another (the allocation's list pass, full Decay's ranking, meshing,
+   the checkpoint classification, the swap lists, ForwardRender's gather, CreatePointCloud, FindVisibleBlocks) on k times the
+   whole GPU's worth of their CTAs (k x SMs x CTAs per SM, whatever the number of tiles; k at most 64). At k = 8 that is more
+   CTAs than the GPU holds at once, so most of them start only after others have retired, and tests can check that the
+   results do not depend on which CTAs are resident. The list pass takes its ticketed form meanwhile, as it does when another
+   engine shares the device. k <= 1 restores the default. */
+void b200_diag_set_grid_scale(b200_engine *e, int k);
+
 /* The IntegrateIntoScene kernel that this engine's last integrate launch ran, and its grid (CTAs): 0 = LDG, 1 = TMA, 2 = V3,
    3 = V4 with two voxels per lane, 4 = V4 with four voxels per lane; + 8 in tolerance mode (B200_INTEGRATE_IMPL=fast).
    -1 and 0 before the first launch. Tests use it to check that the variant they mean to exercise really ran. */
