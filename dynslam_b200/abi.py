@@ -164,7 +164,7 @@ class FrameStats(C.Structure):
                 ("ms_raycast", C.c_float), ("ms_decay", C.c_float), ("ms_total", C.c_float),
                 ("launches", C.c_int64), ("noVisibleBlocks", C.c_int32), ("noIntegratedBlocks", C.c_int32),
                 ("ring_ms_integrate", C.c_float), ("ring_count", C.c_int32), ("totalIntegratedBlocks", C.c_int64),
-                ("droppedSnapshots", C.c_int64)]
+                ("droppedSnapshots", C.c_int64), ("decayReplays", C.c_int64)]
 
 
 # every symbol include/b200fusion.h declares; tests assert the .so exports all of them

@@ -136,6 +136,7 @@ struct DevCounters {
   long long totalIntegrated; // cumulative blocks integrated (never reset; bench reads deltas)
   int integCursor;         // k_integrate_v3: next visible-list item to hand out (dynamic distribution over the persistent grid)
   int integDone;           // k_integrate_v3: CTAs that have stopped claiming; the last one zeroes both for the next launch
+  long long decayReplays;  // partial decay, cumulative: flagged blocks whose reset stores k_decay_commit replayed after the rays
 };
 
 // ---- tile hand-out for kernels whose CTAs wait on one another --------------------------------

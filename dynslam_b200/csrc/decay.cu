@@ -34,41 +34,49 @@ __global__ void __launch_bounds__(256) k_decay_sweep(DecaySweep d) {
   decay_sweep<MODE>(d, (blockIdx.x * blockDim.x + threadIdx.x) >> 5, gridDim.x * (blockDim.x >> 5));
 }
 
-// Partial decay, after everything that reads the voxels: the reset stores of the sweep, then phases 2 + 3 + counters. A warp
-// per item the sweep flagged reloads its block and applies the reset rule again: nothing has written those voxels since the
-// sweep read them, so the rule changes the same voxels to the same bits. The CTA that finishes last commits the pass.
+// Partial decay, after everything that reads the voxels: the reset stores of the sweep and phases 2 + 3 + counters, side by side.
+// The two touch disjoint memory — the replay writes only the voxels of flagged blocks, the commit reads the claims and writes
+// the table, the visibility bytes, the free list and the decay scratch — so neither waits for the other. CTA 0 commits the pass
+// as soon as it is past the dependency wait (a chain of dependent L2 round trips in one CTA, the longer of the two); the other
+// CTAs replay: a warp per item the sweep flagged reloads its block and applies the reset rule again. Nothing has written those
+// voxels since the sweep read them, so the rule changes the same voxels to the same bits. decayItems, which every CTA reads, is
+// cleared by the CTA that finishes last (an arrival count: no CTA waits on another).
 __global__ void __launch_bounds__(256)
 k_decay_commit(b200_voxel *voxels, int maxWeight, const int *resetPtr, b200_hash_entry *table, int numBuckets, const b200_vec3i *ring,
                long long ringCap, const long long *snapStart, int slot, unsigned gen, const unsigned long long *delTag, const int *itemPtr,
                DevCounters *ctr, const int *candList, uint8_t *visType, int *allocList, int *delList, uint8_t *isLeader,
-               unsigned long long *span) {
+               unsigned long long *span, unsigned long long *commitSpan) {
   pdl_wait();            // in the fused frame: the raycast reads the voxels and entries this kernel resets and unlinks
   SpanStamp stamp(span);
-  const int lane = threadIdx.x & 31;
-  const int warps = gridDim.x * (blockDim.x >> 5), warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
-  const int n = ctr->decayItems;
-  for (int item = warp; item < n; item += warps) {
-    const int ptr = resetPtr[item];
-    if (ptr < 0) continue;
-    uint4 *blk = reinterpret_cast<uint4 *>(voxels + (size_t)ptr * BS3) + lane;
-    uint4 raw[8];
-#pragma unroll
-    for (int k = 0; k < 8; ++k) raw[k] = ld_stream(blk + 32 * k);
-    int empty = 0;
-#pragma unroll
-    for (int k = 0; k < 8; ++k) if (decay_reset_pair(raw[k], maxWeight, empty)) st_stream(blk + 32 * k, raw[k]);
-  }
   __shared__ bool lastCta;
   __shared__ unsigned smScan[33];
   __shared__ int smCand[DECAY_CAND_CAP];
-  __threadfence();
+  if (blockIdx.x == 0) {
+    SpanStamp commitStamp(commitSpan);
+    decay_commit_body(table, numBuckets, visType, ring, ringCap, snapStart[slot], itemPtr, delTag, gen, allocList, delList, isLeader, ctr,
+                      candList, smScan, smCand);
+  }
+  const int first = gridDim.x > 1 ? 1 : 0;   // the replaying CTAs: all but CTA 0, or CTA 0 alone on a grid of one
+  if ((int)blockIdx.x >= first) {
+    const int lane = threadIdx.x & 31;
+    const int warps = (gridDim.x - first) * (blockDim.x >> 5), warp = ((blockIdx.x - first) * blockDim.x + threadIdx.x) >> 5;
+    const int n = *(volatile int *)&ctr->decayItems;
+    for (int item = warp; item < n; item += warps) {
+      const int ptr = resetPtr[item];
+      if (ptr < 0) continue;
+      uint4 *blk = reinterpret_cast<uint4 *>(voxels + (size_t)ptr * BS3) + lane;
+      uint4 raw[8];
+#pragma unroll
+      for (int k = 0; k < 8; ++k) raw[k] = ld_stream(blk + 32 * k);
+      int empty = 0;
+#pragma unroll
+      for (int k = 0; k < 8; ++k) if (decay_reset_pair(raw[k], maxWeight, empty)) st_stream(blk + 32 * k, raw[k]);
+    }
+  }
   __syncthreads();
   if (threadIdx.x == 0) lastCta = (atomicAdd(&ctr->decayCtasDone, 1u) == gridDim.x - 1);
   __syncthreads();
-  if (!lastCta) return;
-  __threadfence();
-  decay_commit_body(table, numBuckets, visType, ring, ringCap, snapStart[slot], itemPtr, delTag, gen, allocList, delList, isLeader, ctr,
-                    candList, smScan, smCand);
+  if (lastCta && threadIdx.x == 0) { ctr->decayItems = 0; ctr->decayCtasDone = 0; }
 }
 
 // phase 2: ordered compaction of the claiming items, free-list push by rank (:1072-1073)
@@ -210,7 +218,7 @@ __global__ void k_decay_unlink(b200_hash_entry *table, int numBuckets, uint8_t *
   }
 }
 
-// phases 2 + 3 + counters of a PARTIAL decay, run by the LAST CTA of k_decay_commit — a frame's list is a few thousand items
+// phases 2 + 3 + counters of a PARTIAL decay, run by CTA 0 of k_decay_commit — a frame's list is a few thousand items
 // and the few dozen blocks it empties are known as unordered candidates by then; a launch of its own for this cost 13 us of
 // the frame. Ordered compaction of the claims, leader election, chain unlinking, counter update. All threads of the
 // calling CTA take part; reads of what other CTAs produced go to L2 (__ldcg).
@@ -277,9 +285,7 @@ __device__ void decay_commit_body(b200_hash_entry *table, int numBuckets, uint8_
     ctr->freedLastDecay = nDel;
     ctr->totalDecayed += nDel;
     ctr->decayDeleted = 0;
-    ctr->decayItems = 0;
-    ctr->decayCand = 0;
-    ctr->decayCtasDone = 0;
+    ctr->decayCand = 0;   // (decayItems and decayCtasDone: k_decay_commit's last CTA)
   }
 }
 
@@ -346,7 +352,8 @@ void launch_decay_partial(b200_engine *e, const SceneRef &s, const DecaySweep &d
   launch_chained(fused, k_decay_commit, persistent_grid(e, 2, ((long long)s.numBlocks + 7) / 8), 256, 0, st, s.voxels, d.maxWeight,
                  (const int *)e->d_resetPtr, s.hash, s.numBuckets, (const b200_vec3i *)e->d_ring, e->ringCap, (const long long *)e->d_snapStart,
                  d.slot, d.gen, (const unsigned long long *)e->d_delTag, (const int *)e->d_itemPtr, e->d_ctr, (const int *)e->d_candList,
-                 s.visType, s.allocationList, e->d_delList, e->d_isLeader, fused ? span_slot(e, SPAN_DECAY) : nullptr);
+                 s.visType, s.allocationList, e->d_delList, e->d_isLeader, fused ? span_slot(e, SPAN_DECAY) : nullptr,
+                 fused ? span_slot(e, SPAN_COMMIT) : nullptr);
   trace_end(e, st);
   e->launches++;
 }

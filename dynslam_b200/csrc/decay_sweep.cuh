@@ -76,7 +76,11 @@ DEV void decay_sweep(const DecaySweep &d, int warp, int warps) {
     }
     if (lane == 0) {
       d.itemPtr[item] = claim ? ptr : -1;
-      if (MODE == 0) d.resetPtr[item] = reset ? ptr : -1;
+      if (MODE == 0) {
+        d.resetPtr[item] = reset ? ptr : -1;
+        // diagnostic counter (a hundred or so flagged blocks per pass: an atomic each, no register held across the loop)
+        if (reset) atomicAdd((unsigned long long *)&d.ctr->decayReplays, 1ull);
+      }
       if (claim) {
         atomicMax(&d.delTag[ptr], del_tag(d.gen, (unsigned)item));
         if (MODE == 0) {   // remember the candidate: the commit ranks the few of them instead of scanning the whole list

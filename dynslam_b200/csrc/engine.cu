@@ -685,14 +685,14 @@ static b200_status frame_enqueue(b200_engine *e, b200_scene *s, b200_render_stat
       CK(cudaEventRecord(e->evFork, mainStream));
       CK(cudaStreamWaitEvent(e->sideStream, e->evFork, 0));
       e->stream = e->sideStream;
-      launch_icp(e, g.invM_d, rs->img_w, rs->img_h, s->voxelSize, rs->d_raycastResult, rs->d_raycastImage, d_points, d_normals);
+      launch_icp(e, g.invM_d, rs->img_w, rs->img_h, s->voxelSize, rs->d_raycastResult, rs->d_raycastImage, d_points, d_normals, true);
       if (opts && opts->d_depthRender)   // depth render: ray points and the pose only, nothing of the volume — also beside the decay
         launch_shade(e, r, g.M_d, g.invM_d, rs->img_w, rs->img_h, s->voxelSize, s->maxW, rs->d_raycastResult, nullptr, opts->d_depthRender,
                      B200_RENDER_DEPTH_MAP);
       e->stream = mainStream;
       CK(cudaEventRecord(e->evJoin, e->sideStream));
     } else {
-      launch_icp(e, g.invM_d, rs->img_w, rs->img_h, s->voxelSize, rs->d_raycastResult, rs->d_raycastImage, d_points, d_normals);
+      launch_icp(e, g.invM_d, rs->img_w, rs->img_h, s->voxelSize, rs->d_raycastResult, rs->d_raycastImage, d_points, d_normals, true);
       if (opts && opts->d_depthRender)
         launch_shade(e, r, g.M_d, g.invM_d, rs->img_w, rs->img_h, s->voxelSize, s->maxW, rs->d_raycastResult, nullptr, opts->d_depthRender,
                      B200_RENDER_DEPTH_MAP);
@@ -1024,6 +1024,7 @@ b200_status b200_get_stats(b200_engine *e, b200_frame_stats *out) {
   out->noIntegratedBlocks = e->h_ctr->noIntegrated;
   out->totalIntegratedBlocks = e->h_ctr->totalIntegrated;
   out->droppedSnapshots = e->droppedSnapshots + e->h_ctr->droppedSnapshots;
+  out->decayReplays = e->h_ctr->decayReplays;
   if (e->timingMode >= 2 && e->spanCount > 0) {
     // integrate launch durations from the kernels' own %globaltimer stamps: first CTA past its wait to the last warp's exit
     const int n = e->spanCount;

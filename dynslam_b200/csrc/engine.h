@@ -186,8 +186,9 @@ void launch_raycast(b200_engine *e, const SceneRef &s, const Mat4 &invM, const f
                     float mu, const b200_vec2f *minmax, b200_vec4f *out, bool fused = false, const DecaySweep *sweep = nullptr);
 void launch_shade(b200_engine *e, const SceneRef &s, const Mat4 &M, const Mat4 &invM, int w, int h, float voxelSize, int maxW,
                   const b200_vec4f *rays, b200_vec4u *outChar, float *outDepth, int type);
+// fused = true: the fused frame's ICP pass, stamped in timing modes 3 and 4 (SPAN_ICP)
 void launch_icp(b200_engine *e, const Mat4 &invM, int w, int h, float voxelSize, const b200_vec4f *rays, b200_vec4u *outImg,
-                b200_vec4f *points, b200_vec4f *normals);
+                b200_vec4f *points, b200_vec4f *normals, bool fused = false);
 void launch_forward_render(b200_engine *e, const SceneRef &s, const FrameGeom &g, const float *depth, const b200_vec2f *minmax,
                            const b200_vec4f *rays, b200_vec4f *fwd, int *missing, b200_vec4u *outImg);
 void launch_point_cloud(b200_engine *e, const SceneRef &s, const Mat4 &invM, int w, int h, float voxelSize, int skipPoints,
@@ -259,7 +260,8 @@ static inline void launch_chained(bool chained, void (*kernel)(KArgs...), dim3 g
 
 // %globaltimer spans of the chain's kernels (b200_set_timing modes 2 to 4): one record of SPAN_KERNELS SpanStamp slots per fused
 // frame, SPAN_FRAMES records, zero-filled whenever the mode is set. Mode 2 stamps the integrate kernel only.
-enum { SPAN_MARK, SPAN_SERVE, SPAN_INTEGRATE, SPAN_RAYCAST, SPAN_SWEEP, SPAN_DECAY, SPAN_KERNELS };   // SPAN_RAYCAST: the ray CTAs only
+// SPAN_RAYCAST: the ray CTAs only; SPAN_COMMIT: the commit in CTA 0 of k_decay_commit (rank, elect, unlink, counters); SPAN_ICP: k_icp on the side stream
+enum { SPAN_MARK, SPAN_SERVE, SPAN_INTEGRATE, SPAN_RAYCAST, SPAN_SWEEP, SPAN_DECAY, SPAN_COMMIT, SPAN_ICP, SPAN_KERNELS };
 #define SPAN_FRAMES 8192
 // the slot of kernel k in the record of the fused frame being enqueued, or nullptr when that kernel is not stamped
 static inline unsigned long long *span_slot(const b200_engine *e, int k) {

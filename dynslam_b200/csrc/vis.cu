@@ -404,7 +404,8 @@ DEV void normal_and_angle_img(bool &found, int x, int y, const float4 *__restric
 
 __global__ void __launch_bounds__(256)
 k_icp(const float4 *__restrict__ rays, int w, int h, float voxelSize, float lx, float ly, float lz, uchar4 *outImg, float4 *points,
-      float4 *normals) {
+      float4 *normals, unsigned long long *span) {
+  SpanStamp stamp(span);
   const int x = blockIdx.x * 32 + (threadIdx.x & 31), y = blockIdx.y * 8 + (threadIdx.x >> 5);
   if (x >= w || y >= h) return;
   const int locId = x + y * w;
@@ -422,11 +423,11 @@ k_icp(const float4 *__restrict__ rays, int w, int h, float voxelSize, float lx, 
 }
 
 void launch_icp(b200_engine *e, const Mat4 &invM, int w, int h, float voxelSize, const b200_vec4f *rays, b200_vec4u *outImg,
-                b200_vec4f *points, b200_vec4f *normals) {
+                b200_vec4f *points, b200_vec4f *normals, bool fused) {
   dim3 grid((w + 31) / 32, (h + 7) / 8);
   trace_begin(e, e->stream, "k_icp");
   k_icp<<<grid, 256, 0, e->stream>>>((const float4 *)rays, w, h, voxelSize, -invM.m[8], -invM.m[9], -invM.m[10], (uchar4 *)outImg,
-                                     (float4 *)points, (float4 *)normals);
+                                     (float4 *)points, (float4 *)normals, fused ? span_slot(e, SPAN_ICP) : nullptr);
   trace_end(e, e->stream);
   e->launches++;
 }
@@ -519,7 +520,7 @@ void launch_forward_render(b200_engine *e, const SceneRef &s, const FrameGeom &g
   dim3 grid((g.w + 31) / 32, (g.h + 7) / 8);
   trace_begin(e, st, "k_icp");
   k_icp<<<grid, 256, 0, st>>>((const float4 *)fwd, g.w, g.h, g.voxelSize, -g.invM_d.m[8], -g.invM_d.m[9], -g.invM_d.m[10], (uchar4 *)outImg,
-                              nullptr, nullptr);
+                              nullptr, nullptr, nullptr);
   trace_end(e, st);
   e->launches += 4;
 }

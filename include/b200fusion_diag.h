@@ -20,6 +20,9 @@ typedef struct {
   int32_t ring_count;          /* number of launches measured */
   int64_t totalIntegratedBlocks; /* cumulative blocks integrated since engine creation */
   int64_t droppedSnapshots;    /* decay-queue snapshots dropped because the queue or the ring was full (b200_engine_config) */
+  /* partial Decay since engine creation: blocks with voxels to reset, whose reset stores k_decay_commit made after the sweep
+     (as of the last synchronising call) */
+  int64_t decayReplays;
 } b200_frame_stats;
 
 /* 0 = off; 1 = per-stage CUDA events of the last fused frame (between the chained kernels: they serialise the chain);
@@ -66,8 +69,9 @@ b200_status b200_diag_push_decay_snapshot(b200_engine *e, const b200_vec3i *d_po
 void b200_diag_set_frame_index(b200_engine *e, int32_t f);
 
 /* Kernel spans of the fused frames stamped since b200_set_timing(e, 2 | 3 | 4) (at most 8192 frames, at most maxFrames copied):
-   per frame 6 spans (k_mark_prepare, k_serve_list, the integrate kernel, k_raycast's ray CTAs, the partial decay's sweep, which
-   runs on CTAs of the raycast's grid or as a grid of its own, and k_decay_commit) x {first CTA entry after the kernel's
+   per frame 8 spans (k_mark_prepare, k_serve_list, the integrate kernel, k_raycast's ray CTAs, the partial decay's sweep, which
+   runs on CTAs of the raycast's grid or as a grid of its own, k_decay_commit, the commit that CTA 0 of k_decay_commit runs
+   beside the replay (rank, elect, unlink, counters), and the ICP-map kernel k_icp on the side stream) x {first CTA entry after the kernel's
    dependency wait, last warp exit}, %globaltimer nanoseconds, 0 where the kernel did not run or was not stamped (mode 2 stamps the integrate kernel only). Synchronises the engine's stream; returns the number of frames copied.
    Measurement only. */
 int b200_diag_read_spans(b200_engine *e, unsigned long long *out, int maxFrames);

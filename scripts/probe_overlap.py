@@ -4,8 +4,11 @@ Runs the bench configuration (1242x375 KITTI-shaped stream, 0x60000 blocks, 0x10
 minAge 200, 230-frame pre-roll so partial decay is live, L2 flushed before every frame) and reads the kernels' own %globaltimer
 stamps (b200_set_timing(4), b200_diag_read_spans): per kernel the first CTA's entry after its dependency wait and the last warp's
 exit. The partial decay's sweep runs on CTAs of its own inside the raycast's grid and is stamped apart from the ray CTAs;
-the raycast launch's span covers both. Prints, as medians over the measured frames, each span, the idle time at each of the
-four boundaries between launches (next entry - previous exit) and the frame's chain from the first entry to the last exit.
+the raycast launch's span covers both. The commit that CTA 0 of k_decay_commit runs beside the replay (rank, elect, unlink, counters)
+and the ICP-map kernel on the side stream, which runs beside k_decay_commit, are stamped too. Prints, as medians over the
+measured frames, each span, the idle time at each of the four boundaries between launches (next entry - previous exit), the
+frame's chain from the first entry to the last exit, the frame's tail after the last ray (to the later of the commit's and the
+ICP kernel's exits), and per decay pass the flagged blocks whose reset stores k_decay_commit replayed.
 
 Then mode 3 (an event pair around every launch, which serialises the chain) for the same number of frames: the integrate
 kernel's stamp span against its event pair, launch by launch — the check that the stamps time the integrate launch as the
@@ -19,7 +22,8 @@ import numpy as np, torch
 from dynslam_b200 import engine as E, synth
 import bench
 
-NAMES = ["k_mark_prepare", "k_serve_list", "k_integrate", "k_raycast", "decay sweep", "k_decay_commit"]   # b200_diag_read_spans' slots
+NAMES = ["k_mark_prepare", "k_serve_list", "k_integrate", "k_raycast", "decay sweep", "k_decay_commit", "commit (CTA 0)",
+         "k_icp"]   # b200_diag_read_spans' slots
 CHAIN = ["k_mark_prepare", "k_serve_list", "k_integrate", "k_raycast launch", "k_decay_commit"]             # the launches, in order
 
 
@@ -59,13 +63,17 @@ def main():
     # ---- mode 4: stamps only, the chain as the benchmark runs it ----
     views = [view(frames[idx + i]) for i in range(n)]; idx += n
     torch.cuda.synchronize()
+    eng.sync(rs)
+    st0 = eng.stats()
     eng.set_timing(4)
     for v in views:
         flush.add_(1)
         eng.process_frame_async(rs, v, points, normals, decay=bench.DECAY)
     eng.sync(rs)
+    st1 = eng.stats()
     sp = read_spans(eng, n)
     eng.set_timing(0)
+    replay = (st1.decayReplays - st0.decayReplays) / n
     ok = (sp[:, :, 0] > 0).all(axis=1) & (sp[:, :, 1] > 0).all(axis=1)
     sp = sp[ok]
     us = lambda a: float(np.median(a)) / 1000.0
@@ -79,7 +87,9 @@ def main():
     out.update({"frames": int(ok.sum()), "span_us": spans, "launch_span_us": chain_spans, "idle_us": gaps, "chain_us": chain,
                 "sum_of_spans_us": sum(chain_spans.values()), "sum_of_idle_us": sum(gaps.values()),
                 "sweep_entry_after_raycast_entry_us": us(sp[:, sw, 0] - sp[:, rc, 0]),
-                "sweep_exit_before_raycast_exit_us": us(sp[:, rc, 1] - sp[:, sw, 1])})
+                "sweep_exit_before_raycast_exit_us": us(sp[:, rc, 1] - sp[:, sw, 1]),
+                "tail_after_last_ray_us": us(np.maximum(sp[:, NAMES.index("k_decay_commit"), 1], sp[:, NAMES.index("k_icp"), 1]) - launch[:, 1]),
+                "replays_per_pass": replay})
     print(f"device {props.name}; {int(ok.sum())} frames with every kernel stamped (medians, us)")
     for k, v in spans.items():
         print(f"  span  {k:<20s} {v:7.2f}")
@@ -88,6 +98,8 @@ def main():
     for k, v in gaps.items():
         print(f"  idle  {k:<40s} {v:7.2f}   (negative: the next kernel's first CTA passed its wait before the last warp left)")
     print(f"  chain first entry -> last exit {chain:7.2f}; launch spans {sum(chain_spans.values()):.2f} + idle {sum(gaps.values()):.2f}")
+    print(f"  tail: last ray exit -> later of the commit's and k_icp's exits {out['tail_after_last_ray_us']:7.2f}")
+    print(f"  flagged blocks per decay pass, replayed after the rays: {replay:.1f}")
 
     # ---- mode 3: the integrate kernel's stamps against an event pair around each launch (no overlap: events in the chain) ----
     views = [view(frames[idx + i]) for i in range(n)]; idx += n
