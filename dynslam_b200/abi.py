@@ -159,6 +159,24 @@ class InstanceLayer(C.Structure):
     _fields_ = [("d_color", C.c_void_p), ("d_depth", C.c_void_p), ("tint", C.c_int32 * 4)]
 
 
+class GroupConfig(C.Structure):         # b200_group_config
+    _fields_ = [("static_engine", C.c_void_p), ("static_scene", C.c_void_p), ("static_rs", C.c_void_p),
+                ("static_points", C.c_void_p), ("static_normals", C.c_void_p), ("max_cars", C.c_int32),
+                ("numBlocks", C.c_int32), ("numBuckets", C.c_int32), ("excessSize", C.c_int32), ("voxelSize", C.c_float),
+                ("mu", C.c_float), ("maxW", C.c_int32), ("img_w", C.c_int32), ("img_h", C.c_int32), ("decayRingItems", C.c_int64),
+                ("shared_stream", C.c_int32), ("dim_factor", C.c_float), ("tint_strength", C.c_float)]
+
+
+class GroupImages(C.Structure):         # b200_group_images
+    _fields_ = [("d_instance_rgb", C.c_void_p), ("d_instance_depth", C.c_void_p), ("d_colour_render", C.c_void_p),
+                ("d_depth_render", C.c_void_p), ("d_points", C.c_void_p), ("d_normals", C.c_void_p)]
+
+
+class GroupCar(C.Structure):            # b200_group_car
+    _fields_ = [("slot", C.c_int32), ("action", C.c_int32), ("copy_mask", Mask), ("delete_mask", Mask), ("cam", Camera),
+                ("fuse", C.c_int32), ("tint", C.c_int32 * 4)]
+
+
 class FrameStats(C.Structure):
     _fields_ = [("ms_allocate", C.c_float), ("ms_integrate", C.c_float), ("ms_expected", C.c_float),
                 ("ms_raycast", C.c_float), ("ms_decay", C.c_float), ("ms_total", C.c_float),
@@ -184,6 +202,8 @@ EXPORTS = [
     "b200_mesh_scene", "b200_checkpoint_save", "b200_checkpoint_load", "b200_comm_unique_id", "b200_comm_create", "b200_comm_destroy", "b200_comm_last_error", "b200_gather_composite_submit",
     "b200_gather_composite_release", "b200_gather_composite_wait",
     "b200_render_view_async", "b200_render_view_sync", "b200_render_view_submit", "b200_render_view_wait", "b200_engine_wait_engine",
+    "b200_volume_restart_async", "b200_group_create", "b200_group_destroy", "b200_group_last_error", "b200_group_slot",
+    "b200_group_slot_images", "b200_group_track_start", "b200_group_frame_async", "b200_group_sync",
 ]
 # measurement / test hooks (include/b200fusion_diag.h): exported by the same library, not part of the drop-in boundary
 DIAG_EXPORTS = ["b200_set_timing", "b200_get_trace", "b200_get_stats", "b200_selftest_divide", "b200_diag_set_max_rendering_blocks", "b200_diag_set_grid_scale",
@@ -270,6 +290,17 @@ def load_library():
     lib.b200_render_view_submit.argtypes = [vp, P(Scene), P(RenderState), P(Camera), C.c_int, vp, vp, C.c_int]
     lib.b200_render_view_wait.argtypes = [vp, C.c_int]
     lib.b200_engine_wait_engine.argtypes = [vp, vp]
+    lib.b200_volume_restart_async.argtypes = [vp, P(Scene), P(RenderState)]
+    lib.b200_group_create.argtypes = [P(GroupConfig), P(vp)]
+    lib.b200_group_destroy.argtypes = [vp]
+    lib.b200_group_destroy.restype = None
+    lib.b200_group_last_error.argtypes = [vp]
+    lib.b200_group_last_error.restype = C.c_char_p
+    lib.b200_group_slot.argtypes = [vp, C.c_int, P(vp), P(P(Scene)), P(P(RenderState))]
+    lib.b200_group_slot_images.argtypes = [vp, C.c_int, P(GroupImages)]
+    lib.b200_group_track_start.argtypes = [vp, C.c_int]
+    lib.b200_group_frame_async.argtypes = [vp, vp, vp, P(View), P(GroupCar), C.c_int, P(C.c_int32), vp, vp]
+    lib.b200_group_sync.argtypes = [vp]
     lib.b200_set_timing.argtypes = [vp, C.c_int]
     lib.b200_set_timing.restype = None
     lib.b200_get_stats.argtypes = [vp, P(FrameStats)]

@@ -342,6 +342,59 @@ b200_status b200_reset_scene(b200_engine *e, b200_scene *s) {
   return download_sync(e, s, nullptr);
 }
 
+// What b200_engine_create, a new scene reset by b200_reset_scene and a new (zeroed) render state start from, stream-ordered on
+// e's stream. Cleared: what engine_create clears and a later call reads before it writes. The scratch create leaves
+// uninitialised (ring items, per-item scratch, block records) is written before it is read. The scan descriptors (d_scanDesc,
+// d_meshDesc) and the decay tags (d_delTag) are tagged with the engine's generation counters, which keep counting across the
+// restart, so nothing left in them can match a later pass; the allocation's request keys are tagged with the frame index,
+// which restarts at 0, so they are cleared (as b200_checkpoint_load clears them).
+b200_status b200_volume_restart_async(b200_engine *e, b200_scene *s, b200_render_state *rs) {
+  if (!e) return B200_ERR_INVALID;
+  b200_status st = check_scene(e, s); if (st) return st;
+  if (!rs || !rs->d_visibleBlockPositions || !rs->d_entriesVisibleType || !rs->d_minmax || !rs->d_raycastResult || !rs->d_raycastImage ||
+      rs->img_w <= 0 || rs->img_h <= 0) {
+    snprintf(e->err, sizeof(e->err), "volume_restart: render state or one of its buffers missing"); return B200_ERR_INVALID;
+  }
+  if ((e->copyStream && (e->slotBusy[0] || e->slotBusy[1])) || preview_slot_busy(e)) {
+    snprintf(e->err, sizeof(e->err), "volume_restart: a host-frame or preview slot is still outstanding (wait for it first)");
+    return B200_ERR_INVALID;
+  }
+  CK(cudaSetDevice(e->device));
+  const cudaStream_t q = e->stream;
+  const size_t px = (size_t)rs->img_w * rs->img_h, noTotal = (size_t)e->noTotal;
+  // engine scratch, as engine_create leaves it
+  CK(cudaMemsetAsync(e->d_ctr, 0, sizeof(DevCounters), q));
+  CK(cudaMemsetAsync(e->d_reqKey, 0, sizeof(unsigned long long) * noTotal, q));
+  CK(cudaMemsetAsync(e->d_reqBits, 0, sizeof(unsigned) * (size_t)e->noWords * 2, q));
+  CK(cudaMemsetAsync(e->d_markBytes, 0, noTotal, q));
+  CK(cudaMemsetAsync(e->d_snapCount, 0, sizeof(int) * SNAP_SLOTS, q));
+  CK(cudaMemsetAsync(e->d_snapStart, 0, sizeof(long long) * SNAP_SLOTS, q));
+  // the scene: b200_reset_scene's kernel (it also sets the free-list counters); swap states as a new scene has them
+  launch_reset(e, scene_ref(s, nullptr));
+  if (s->d_swapStates) CK(cudaMemsetAsync(s->d_swapStates, 0, noTotal, q));
+  // the render state, zeroed as a newly allocated one is
+  CK(cudaMemsetAsync(rs->d_visibleBlockPositions, 0, sizeof(b200_vec3i) * (size_t)s->numBlocks, q));
+  CK(cudaMemsetAsync(rs->d_entriesVisibleType, 0, noTotal, q));
+  CK(cudaMemsetAsync(rs->d_minmax, 0, sizeof(b200_vec2f) * px, q));
+  CK(cudaMemsetAsync(rs->d_raycastResult, 0, sizeof(b200_vec4f) * px, q));
+  CK(cudaMemsetAsync(rs->d_raycastImage, 0, sizeof(b200_vec4u) * px, q));
+  if (rs->d_forwardProjection) CK(cudaMemsetAsync(rs->d_forwardProjection, 0, sizeof(b200_vec4f) * px, q));
+  if (rs->d_fwdProjMissingPoints) CK(cudaMemsetAsync(rs->d_fwdProjMissingPoints, 0, sizeof(int32_t) * px, q));
+  CK(cudaGetLastError());
+  // host state of a new engine
+  e->frameIdx = 0;
+  e->qHead = 0; e->qSize = 0; e->droppedSnapshots = 0;
+  e->totalDecayed = 0; e->lastNoIntegrated = 0;
+  e->deadPending = false;
+  e->ptrListFor = nullptr; e->tableVersion++;   // (launch_reset counted a launch: a checkpoint save classifies afresh)
+  // The device counters are the reset ones; the host fields get the same values now, and b200_sync() refreshes them as usual.
+  // The device copy stays authoritative so that nothing uploads host counters over it before then.
+  e->hostAuthoritative = false;
+  s->lastFreeBlockId = s->numBlocks - 1; s->lastFreeExcessListId = s->excessSize - 1;
+  rs->noVisibleBlocks = 0; rs->noFwdProjMissingPoints = 0;
+  return B200_OK;
+}
+
 // Host half of a decay-queue push: the slot the next snapshot goes to, now counted in the queue. The reference's queue of
 // visible-list copies is unbounded (Reco_CUDA.cu:302-317); this one has SNAP_SLOTS frame slots and a ring of list items.
 // When Decay() is never called (--voxel_decay=false) or min_decay_age is very large, the OLDEST snapshot is dropped to make

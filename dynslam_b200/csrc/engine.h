@@ -121,6 +121,7 @@ b200_status download_sync(b200_engine *e, b200_scene *s, b200_render_state *rs);
 extern "C" int push_snapshot_slot(b200_engine *e);   // (defined inside engine.cu's extern "C" block)
 void checkpoint_release(b200_engine *e);
 void preview_release(b200_engine *e);
+bool preview_slot_busy(const b200_engine *e);   // a b200_render_view_submit slot not yet waited for
 
 #define SNAP_SLOTS 4096
 

@@ -82,6 +82,8 @@ void preview_release(b200_engine *e) {
   e->pv = nullptr;
 }
 
+bool preview_slot_busy(const b200_engine *e) { return e->pv && (e->pv->busy[0] || e->pv->busy[1]); }
+
 // every rejection of b200_render_view_async / _submit, before anything is allocated or enqueued
 static b200_status check_view(b200_engine *e, const b200_scene *s, const b200_render_state *rs, const b200_camera *cam, int type,
                               const void *outChar, const void *outDepth) {

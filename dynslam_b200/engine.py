@@ -260,6 +260,12 @@ class Engine:
         self.after_torch()
         self.check(self.lib.b200_checkpoint_load(self.h, C.byref(scene.c), C.byref(renderState.c), b.ctypes.data, b.size))
 
+    def restart_volume(self, scene, renderState):
+        """b200_volume_restart_async: on this engine's stream, with no host wait and no allocation, the engine, scene and render
+        state become what a newly created engine on a newly allocated, reset scene with a new render state is (frame index 0)."""
+        self.after_torch()
+        self.check(self.lib.b200_volume_restart_async(self.h, C.byref(scene.c), C.byref(renderState.c)))
+
     def set_frame_index(self, f):
         """test hook (include/b200fusion_diag.h): the frame index Decay measures block ages against"""
         self.lib.b200_diag_set_frame_index(self.h, int(f))
@@ -730,3 +736,180 @@ class SwappingEngine:
                 if has[i]:
                     cache.stored[int(entry)] = blocks[i].copy()
         return n
+
+
+class _DeviceBuffer:
+    """a device allocation the library owns, seen by torch without a copy (__cuda_array_interface__)"""
+
+    def __init__(self, ptr, n, typestr):
+        self.__cuda_array_interface__ = {"shape": (n,), "typestr": typestr, "data": (ptr, False), "version": 3, "strides": None}
+
+
+def _device_view(ptr, n, dtype, device):
+    typestr = {torch.uint8: "|u1", torch.int32: "<i4", torch.float32: "<f4"}[dtype]
+    return torch.as_tensor(_DeviceBuffer(ptr, n, typestr), device=device)
+
+
+class _SlotScene:
+    """a group slot's scene: the group's b200_scene and views of its buffers"""
+
+    def __init__(self, cptr, device):
+        self.c = cptr.contents
+        self.device = device
+        self.numBlocks, self.numBuckets, self.excessSize = self.c.numBlocks, self.c.numBuckets, self.c.excessSize
+        self.noTotalEntries = self.numBuckets + self.excessSize
+        self.params = SceneParams(voxelSize=self.c.voxelSize, mu=self.c.mu, maxW=self.c.maxW)
+
+    @property
+    def lastFreeBlockId(self):
+        return self.c.lastFreeBlockId
+
+    @property
+    def lastFreeExcessListId(self):
+        return self.c.lastFreeExcessListId
+
+
+class _SlotRenderState:
+    """a group slot's render state: the group's b200_render_state and views of its buffers"""
+
+    def __init__(self, cptr, scene, device):
+        r = cptr.contents
+        self.c, self.w, self.h = r, r.img_w, r.img_h
+        px = r.img_w * r.img_h
+        self.visibleBlockPositions = _device_view(r.d_visibleBlockPositions, scene.numBlocks * 3, torch.int32, device)
+        self.entriesVisibleType = _device_view(r.d_entriesVisibleType, scene.noTotalEntries, torch.uint8, device)
+        self.renderingRangeImage = _device_view(r.d_minmax, px * 2, torch.float32, device)
+        self.raycastResult = _device_view(r.d_raycastResult, px * 4, torch.float32, device)
+        self.raycastImage = _device_view(r.d_raycastImage, px * 4, torch.uint8, device)
+
+    @property
+    def noVisibleBlocks(self):
+        return self.c.noVisibleBlocks
+
+
+class _SlotEngine(Engine):
+    """a group slot's engine: every Engine method works on it; the group owns and destroys it"""
+
+    def __init__(self, lib, handle, scene):
+        self.lib, self.h, self.scene = lib, C.c_void_p(handle), scene
+        self._ext = torch.cuda.ExternalStream(self.lib.b200_engine_stream(self.h), device=scene.device)
+
+    def close(self):
+        self.h = None
+
+
+class VolumeSlot:
+    """one slot of a VolumeGroup: its engine, scene, render state and images (torch views of the group's buffers)"""
+
+    def __init__(self, group, i):
+        lib, dev = group.lib, group.device
+        eng, sc, rs = C.c_void_p(), C.POINTER(abi.Scene)(), C.POINTER(abi.RenderState)()
+        group.check(lib.b200_group_slot(group.h, i, C.byref(eng), C.byref(sc), C.byref(rs)))
+        im = abi.GroupImages()
+        group.check(lib.b200_group_slot_images(group.h, i, C.byref(im)))
+        self.scene = _SlotScene(sc, dev)
+        self.engine = _SlotEngine(lib, eng.value, self.scene)
+        self.rs = _SlotRenderState(rs, self.scene, dev)
+        px = self.rs.w * self.rs.h
+        self.instance_rgb = _device_view(im.d_instance_rgb, px * 4, torch.uint8, dev)
+        self.instance_depth = _device_view(im.d_instance_depth, px, torch.float32, dev)
+        self.colour_render = _device_view(im.d_colour_render, px * 4, torch.uint8, dev)
+        self.depth_render = _device_view(im.d_depth_render, px, torch.float32, dev)
+        self.points = _device_view(im.d_points, px * 4, torch.float32, dev)
+        self.normals = _device_view(im.d_normals, px * 4, torch.float32, dev)
+
+
+class GroupCar:
+    """one car of a VolumeGroup frame (b200_group_car): its slot, silhouette action and masks (make_mask), pose, depth
+    intrinsics, whether it is fused, and its layer's tint. prepare() builds the C array once for reuse."""
+
+    def __init__(self, slot, action, copy_mask, delete_mask, M, proj, fuse=True, tint=(0, 0, 0, 255)):
+        self.slot, self.action, self.copy_mask, self.delete_mask = slot, action, copy_mask, delete_mask
+        self.M, self.proj, self.fuse, self.tint = M, proj, fuse, tint
+
+
+class VolumeGroup:
+    """b200_group_*: the static map (an Engine, its Scene and live RenderStateVH) and max_cars car-volume slots created up front
+    (include/b200fusion.h, "volume group"). frame() enqueues DynSLAM's whole multi-volume frame as one call; track_start(i)
+    restarts slot i for a new track on the device. slots[i] gives each slot's Engine, scene, render state and images, on which
+    every per-engine call works."""
+
+    def __init__(self, static_engine, static_rs, static_points, static_normals, max_cars, shared_stream=False, numBlocks=0,
+                 numBuckets=0, excessSize=0, voxelSize=0.0, mu=0.0, maxW=0, decayRingItems=0, dim_factor=0.10, tint_strength=1.0):
+        self.lib = static_engine.lib
+        self.static, self.static_rs = static_engine, static_rs
+        self.device = static_engine.scene.device
+        self._keep = (static_points, static_normals)
+        cfg = abi.GroupConfig()
+        cfg.static_engine = static_engine.h.value
+        cfg.static_scene = C.addressof(static_engine.scene.c)
+        cfg.static_rs = C.addressof(static_rs.c)
+        cfg.static_points, cfg.static_normals = _ptr(static_points), _ptr(static_normals)
+        cfg.max_cars = max_cars
+        cfg.numBlocks, cfg.numBuckets, cfg.excessSize = numBlocks, numBuckets, excessSize
+        cfg.voxelSize, cfg.mu, cfg.maxW = voxelSize, mu, maxW
+        cfg.decayRingItems, cfg.shared_stream = decayRingItems, int(shared_stream)
+        cfg.dim_factor, cfg.tint_strength = dim_factor, tint_strength
+        static_engine.after_torch()
+        h = C.c_void_p()
+        rc = self.lib.b200_group_create(C.byref(cfg), C.byref(h))
+        self.h = h if rc == abi.OK else None
+        if rc:
+            msg = self.lib.b200_group_last_error(None).decode()
+            raise (CudaError if rc == abi.ERR_CUDA else ValueError)(msg)
+        self.max_cars = max_cars
+        self.slots = [VolumeSlot(self, i) for i in range(max_cars)]
+
+    def check(self, rc):
+        if rc == abi.OK:
+            return
+        msg = self.lib.b200_group_last_error(self.h).decode()
+        if rc in (abi.ERR_VBA_FULL, abi.ERR_EXCESS_FULL):
+            raise RuntimeError(msg)
+        raise (CudaError if rc == abi.ERR_CUDA else ValueError)(msg)
+
+    def close(self):
+        if getattr(self, "h", None):
+            self.lib.b200_group_destroy(self.h)
+            self.h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def track_start(self, slot):
+        """b200_group_track_start: slot's volume restarted for a new track, after everything the group enqueued so far"""
+        self.static.after_torch()
+        self.check(self.lib.b200_group_track_start(self.h, int(slot)))
+
+    @staticmethod
+    def prepare(cars):
+        """the b200_group_car array of a list of GroupCar (build it once for a frame enqueued more than once)"""
+        arr = (abi.GroupCar * max(len(cars), 1))()
+        for k, c in enumerate(cars):
+            a = arr[k]
+            a.slot, a.action, a.fuse = int(c.slot), int(c.action), int(bool(c.fuse))
+            if c.copy_mask is not None:
+                a.copy_mask = c.copy_mask
+            if c.delete_mask is not None:
+                a.delete_mask = c.delete_mask
+            a.cam = make_camera(c.M, c.proj)
+            a.tint = (C.c_int32 * 4)(*[int(t) for t in c.tint])
+        return arr, len(cars)
+
+    def frame(self, rgb, depth, static_view, cars, out_color, out_depth, decay=None, wait_inputs=True):
+        """b200_group_frame_async. cars: a list of GroupCar or prepare()'s result. rgb / depth: the frame, updated in place by the
+        silhouettes; static_view normally views them. wait_inputs=False: the caller already orders the tensors on the static
+        engine's stream."""
+        arr, n = cars if isinstance(cars, tuple) else self.prepare(cars)
+        dec = (C.c_int32 * 2)(int(decay[0]), int(decay[1])) if decay is not None else None
+        if wait_inputs:
+            self.static.after_torch()
+        self.check(self.lib.b200_group_frame_async(self.h, _ptr(rgb), _ptr(depth), C.byref(static_view.c), arr, n, dec, _ptr(out_color),
+                                                   _ptr(out_depth)))
+
+    def sync(self):
+        """b200_group_sync: host counters of the static map and of every slot"""
+        self.check(self.lib.b200_group_sync(self.h))

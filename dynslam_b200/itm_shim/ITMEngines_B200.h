@@ -184,6 +184,17 @@ class ITMSceneReconstructionEngine_B200<TVoxel, ITMVoxelBlockHash> : public ITMS
     b200_detail::UnpackScene(s, scene);
   }
 
+  /// What a new InfiniTamDriver for a new track would be, without building one: the engine, scene and render state behave like a
+  /// newly created engine on a newly allocated, reset scene with a new render state (frame index 0, empty decay queue).
+  /// Stream-ordered on the engine's stream; the host waits for nothing and nothing is allocated (b200_volume_restart_async).
+  void RestartScene(ITMScene<TVoxel, ITMVoxelBlockHash> *scene, ITMRenderState *renderState) {
+    b200_scene s = b200_detail::PackScene(scene);
+    b200_render_state r = b200_detail::PackRenderState(renderState);
+    h->check(b200_volume_restart_async(h->e, &s, &r));
+    b200_detail::UnpackScene(s, scene);
+    b200_detail::UnpackRenderState(r, renderState);
+  }
+
   void AllocateSceneFromDepth(ITMScene<TVoxel, ITMVoxelBlockHash> *scene, const ITMView *view, const ITMTrackingState *trackingState,
                               const ITMRenderState *renderState, bool onlyUpdateVisibleList = false) override {
     b200_scene s = b200_detail::PackScene(scene);

@@ -5,6 +5,9 @@ One engine per volume. With shared_stream=True every engine runs on one stream (
 engine has a stream of its own and the frame forks and joins through b200_engine_wait_engine, so the volumes fuse concurrently
 (include/b200fusion.h, at the engine handle; INTEGRATION.md, "Static map and car volumes on one GPU"). Both forms compute the
 same bytes.
+
+StreetVolumes makes each call of that sequence from Python; GroupStreetVolumes enqueues the same frame as one call of a volume
+group (b200_group_frame_async), whose car volumes are slots created up front and restarted on the device for a new track.
 """
 import numpy as np
 import torch
@@ -46,12 +49,14 @@ class DeviceFrame:
         self.M, self.proj, self.index = M, proj, index
         self.car_poses = [car.object_pose(index, M) for car in cars]
         self.keep, ops = [], []
+        self.masks = [None] * len(masks)          # per car: its b200_mask, or None when it is not in the frame
         for k, m in enumerate(masks):
             if m is None:
                 continue
             t = torch.from_numpy(m[1]).to(device)
             self.keep.append(t)
             mk = E.make_mask(m[0], t)
+            self.masks[k] = mk
             ops.append((E.EXTRACT, mk, mk, inst_rgb[k], inst_depth[k]))
         self.ops = E.InstanceFrames.prepare_ops(ops) if ops else None
 
@@ -151,3 +156,96 @@ class StreetVolumes:
     def close(self):
         for eng in self.engines:
             eng.close()
+
+
+class GroupStreetVolumes:
+    """StreetVolumes' volumes and frames through a volume group (E.VolumeGroup): the static map is an engine of its own, the
+    `ncars` car volumes are slots 0 .. ncars-1 of the group, started at construction. step(fr) is one b200_group_frame_async
+    after the two copies of the input frame; state(i) gives the same bytes as StreetVolumes.state(i) for the same frames."""
+
+    def __init__(self, ncars, w, h, shared_stream, device="cuda:0", decay=DECAY, static_blocks=STATIC_BLOCKS,
+                 car_blocks=CAR_BLOCKS, num_buckets=NUM_BUCKETS, excess=EXCESS, max_cars=None):
+        dev = torch.device(device)
+        self.dev, self.w, self.h, self.decay, self.ncars = dev, w, h, decay, ncars
+        self.stream = torch.cuda.Stream(device=dev)
+        with torch.cuda.stream(self.stream):
+            self.static_scene = E.Scene(E.SceneParams(), static_blocks, num_buckets, excess, device=device)
+            self.static = E.Engine(self.static_scene, (w, h), stream=self.stream.cuda_stream)
+            E.SceneReconstructionEngine(self.static).ResetScene(self.static_scene)
+            self.static_rs = E.VisualisationEngine(self.static, self.static_scene).CreateRenderState((w, h))
+            self.static_points = torch.zeros(h * w * 4, dtype=torch.float32, device=dev)
+            self.static_normals = torch.zeros(h * w * 4, dtype=torch.float32, device=dev)
+            self.frame_rgb = torch.zeros((h, w, 4), dtype=torch.uint8, device=dev)
+            self.frame_depth = torch.zeros((h, w), dtype=torch.float32, device=dev)
+            self.out_color = torch.zeros((h, w, 4), dtype=torch.uint8, device=dev)
+            self.out_depth = torch.zeros((h, w), dtype=torch.float32, device=dev)
+        torch.cuda.synchronize(dev)
+        self.group = E.VolumeGroup(self.static, self.static_rs, self.static_points, self.static_normals,
+                                   ncars if max_cars is None else max_cars, shared_stream=shared_stream, numBlocks=car_blocks,
+                                   numBuckets=num_buckets, excessSize=excess, voxelSize=0.035, mu=1.0, maxW=50)
+        for k in range(ncars):
+            self.group.track_start(k)
+        self.static_view = E.View(self.frame_depth, self.frame_rgb, np.eye(4, dtype=np.float32), synth.kitti_intrinsics())
+        self._cars = [synth.FollowedCar(i, seed=3) for i in range(ncars)]
+
+    def upload(self, frames, first=0):
+        """device-resident copies of host frames (street_frames), as StreetVolumes.upload makes them"""
+        return [DeviceFrame(fr, first + i, self._cars, [None] * self.ncars, [None] * self.ncars, self.dev)
+                for i, fr in enumerate(frames)]
+
+    def cars(self, fr, plan=None):
+        """the GroupCar list of frame fr: car k in slot k, extracted when it is in the frame, fused, with TINTS[k]. plan (optional):
+        per car, (action, fuse) replacing that default, or None to leave the car out of the frame"""
+        out = []
+        for k in range(self.ncars):
+            action, fuse = (E.EXTRACT if fr.masks[k] is not None else E.KEEP), True
+            if plan is not None:
+                if plan[k] is None:
+                    continue
+                action, fuse = plan[k]
+            m = fr.masks[k] if action != E.KEEP else None
+            out.append(E.GroupCar(k, action, m, m, fr.car_poses[k], fr.proj, fuse=fuse, tint=TINTS[k % len(TINTS)]))
+        return out
+
+    def prepare(self, fr, plan=None):
+        """(fr, the prepared b200_group_car array): enqueued by step without building the array again"""
+        return fr, E.VolumeGroup.prepare(self.cars(fr, plan))
+
+    def step(self, fr, plan=None):
+        """enqueue one frame of every volume: the two copies of the input frame and one b200_group_frame_async; no host
+        synchronisation. fr: a DeviceFrame or prepare()'s result"""
+        fr, cars = fr if isinstance(fr, tuple) else self.prepare(fr, plan)
+        with torch.cuda.stream(self.stream):
+            self.frame_depth.copy_(fr.depth)
+            self.frame_rgb.copy_(fr.rgb)
+            self.static_view.set_pose(fr.M)
+            self.static_view.c.proj_d = self.static_view.c.proj_rgb = E.abi.f4(*[float(x) for x in fr.proj])
+            self.group.frame(self.frame_rgb, self.frame_depth, self.static_view, cars, self.out_color, self.out_depth, decay=self.decay,
+                             wait_inputs=False)
+
+    def track_start(self, slot):
+        with torch.cuda.stream(self.stream):
+            self.group.track_start(slot)
+
+    def synchronize(self):
+        self.stream.synchronize()
+        self.group.sync()
+
+    def volume(self, i):
+        """(engine, scene, render state, points, normals) of volume i: 0 the static map, 1 + k car k's slot"""
+        if i == 0:
+            return self.static, self.static_scene, self.static_rs, self.static_points, self.static_normals
+        sl = self.group.slots[i - 1]
+        return sl.engine, sl.scene, sl.rs, sl.points, sl.normals
+
+    def state(self, i):
+        """the bytes of volume i, as StreetVolumes.state(i) gives them"""
+        eng, sc, rs, points, normals = self.volume(i)
+        ck = eng.save_checkpoint(sc, rs)
+        return {"checkpoint": ck, "rays": rs.raycastResult.cpu().numpy().tobytes(),
+                "image": rs.raycastImage.view(self.h, self.w, 4).cpu().numpy().tobytes(),
+                "points": points.cpu().numpy().tobytes(), "normals": normals.cpu().numpy().tobytes()}
+
+    def close(self):
+        self.group.close()
+        self.static.close()

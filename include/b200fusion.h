@@ -152,7 +152,8 @@ typedef enum {                 /* IITMVisualisationEngine::RenderImageType, Vis.
      3. b200_process_frame_async of the static map;
      4. b200_engine_wait_engine(static, car) for every car, then b200_composite_instances on the static engine.
    Stand-alone calls (b200_decay with forceAllVoxels for Reap, b200_mesh_scene, b200_checkpoint_save) on one engine may run
-   while the other engines' frames are in flight; they wait for their own engine's stream only. */
+   while the other engines' frames are in flight; they wait for their own engine's stream only. The volume group (b200_group_*,
+   below) enqueues this sequence as one call and keeps the car volumes in a pool of slots restarted on the device. */
 typedef struct b200_engine b200_engine;
 
 typedef struct {
@@ -181,6 +182,19 @@ int32_t b200_frame_index(const b200_engine *e);      /* frameIdx, Reco_CUDA.h:37
 
 /* ResetScene — Reco_CUDA.cu:145-172 */
 b200_status b200_reset_scene(b200_engine *e, b200_scene *scene);
+/* Restart a volume on the device (no reference twin: what a new InfiniTamDriver for a new track would be). Afterwards e, scene
+   and rs behave byte for byte like a newly created engine on a newly allocated scene that b200_reset_scene reset, with a newly
+   allocated (zeroed) render state: frame index 0; decay queue and ring empty; decayed total and dropped-snapshot count 0;
+   allocation request keys (tagged with frame indices) cleared; hash table, voxel blocks, free lists and counters reset as
+   ResetScene resets them, swap states zeroed; every buffer of rs zeroed (entriesVisibleType, the visible list, the images,
+   the forward-projection buffers when present) and noVisibleBlocks 0. Unlike b200_reset_scene, which keeps the frame index as
+   the reference's ResetScene does, the frame index restarts.
+   Stream-ordered on e's stream: no host wait, no allocation, only memsets and one reset kernel, so it may be enqueued while
+   other engines' frames are in flight and inside a stream capture. The host fields of scene and rs are set to the reset
+   values; b200_sync() refreshes them as usual. B200_ERR_INVALID, with nothing enqueued: a scene that does not fit the engine,
+   rs or one of its buffers missing, a host-frame slot (b200_host_frame_submit*) or a preview slot (b200_render_view_submit)
+   not yet waited for. */
+b200_status b200_volume_restart_async(b200_engine *e, b200_scene *scene, b200_render_state *rs);
 /* AllocateSceneFromDepth — Reco_CUDA.cu:175-358 */
 b200_status b200_allocate_from_depth(b200_engine *e, b200_scene *scene, b200_render_state *rs,
                                      const b200_view *view, int onlyUpdateVisibleList);
@@ -457,6 +471,85 @@ b200_status b200_composite_color(b200_engine *e, b200_vec4u *d_target_color, flo
 b200_status b200_composite_instances(b200_engine *e, b200_vec4u *d_out_color, float *d_out_depth, int n,
                                      const b200_instance_layer *layers, int n_layers, float dim_factor,
                                      float tint_strength);
+
+/* ---- volume group: the static map and a pool of car-volume slots on one GPU (InstanceReconstructor's one ITMScene per car
+   track, DS/InstRecLib/InstanceReconstructor.cpp:363-389) --------------------------------------------------------------------
+   b200_group_create makes max_cars slots up front, each with an engine, a scene, a render state, an instance frame (RGBA8 and
+   f32 depth), a colour and a depth render for the composite and the ICP point and normal maps. So the device waits of
+   b200_engine_create happen there only, and slot engines are destroyed only by b200_group_destroy: a track that starts takes a
+   slot and restarts it on the device (b200_group_track_start), a track that ends leaves its slot for the next one.
+   Memory per slot (arithmetic from the buffer sizes, not a measurement), at the defaults and a 1242 x 375 image: voxel blocks
+   29.3 MB, hash table 31.5 MB, excess and allocation lists 2.1 MB, visibility bytes 1.6 MB, the render state's images 13.0 MB,
+   instance frame and renders 7.5 MB, ICP maps 14.9 MB, engine scratch about 19 MB: about 119 MB.
+
+   Every per-engine call works on a slot's engine, scene and render state (b200_group_slot) unchanged: b200_decay with
+   forceAllVoxels for Reap, b200_mesh_scene, b200_checkpoint_save / _load, b200_render_view_async. They are ordered after the
+   slot's own work only, as between any engines. */
+typedef struct b200_group b200_group;
+
+typedef struct {
+  b200_engine *static_engine;          /* the caller's static map: engine, scene and live render state, kept by pointer for the */
+  b200_scene *static_scene;            /* group's life; its host counters are written by b200_group_sync */
+  b200_render_state *static_rs;
+  b200_vec4f *static_points, *static_normals;   /* the static map's ICP maps (w*h each) */
+  int32_t max_cars;                    /* slots */
+  /* the car volumes; a field <= 0 takes the default in brackets (bench.py configs[2]: InstanceReconstructor.cpp:365-389's
+     5 x 5 x 10 m at 0.035 m, with the full-size table) */
+  int32_t numBlocks;                   /* [7142] */
+  int32_t numBuckets, excessSize;      /* [0x100000, 0x80000] */
+  float voxelSize, mu;                 /* [0.035, 1.0]; viewFrustum and stopIntegratingAtMaxW are the static scene's */
+  int32_t maxW;                        /* [50] */
+  int32_t img_w, img_h;                /* [the static render state's]; must equal it */
+  int64_t decayRingItems;              /* as b200_engine_config's [24 x numBlocks] */
+  int32_t shared_stream;               /* 1: every slot on the static engine's stream; 0: a stream per slot */
+  float dim_factor, tint_strength;     /* the composite's, as b200_composite_instances takes them */
+} b200_group_config;
+
+typedef struct {                       /* a slot's device images, owned by the group (img_w x img_h each) */
+  b200_vec4u *d_instance_rgb; float *d_instance_depth;   /* the instance frame the silhouettes cut out */
+  b200_vec4u *d_colour_render; float *d_depth_render;    /* RENDER_COLOUR_FROM_VOLUME and RENDER_DEPTH_MAP of its latest frame */
+  b200_vec4f *d_points, *d_normals;                      /* its ICP maps */
+} b200_group_images;
+
+typedef struct {                       /* one car of a frame */
+  int32_t slot;
+  int32_t action;                      /* b200_silhouette_op.action, with its masks (device data, the caller's) */
+  b200_mask copy_mask, delete_mask;
+  b200_camera cam;                     /* the car's pose (M and its inverse) and the depth intrinsics of its instance frame */
+  int32_t fuse;                        /* nonzero: fuse the instance frame into the slot's volume and composite its layer */
+  int32_t tint[4];                     /* the layer's tint (kMatplotlib2Palette[track id % 10] in DynSLAM) */
+} b200_group_car;
+
+/* On failure nothing is left allocated, *out is NULL and b200_group_last_error(NULL) gives the reason (thread-local). Waits for
+   the device. */
+b200_status b200_group_create(const b200_group_config *cfg, b200_group **out);
+void b200_group_destroy(b200_group *g);
+const char *b200_group_last_error(const b200_group *g);
+/* slot i's engine, scene and render state (pointers into the group; any output may be NULL) */
+b200_status b200_group_slot(b200_group *g, int slot, b200_engine **engine, b200_scene **scene, b200_render_state **rs);
+b200_status b200_group_slot_images(b200_group *g, int slot, b200_group_images *out);
+/* A new track in slot: b200_volume_restart_async of the slot's volume on its stream, after everything the group has enqueued
+   so far (the slot's stream waits for the static engine's). No host wait, no allocation. */
+b200_status b200_group_track_start(b200_group *g, int slot);
+/* One frame of every volume as one enqueue, DynSLAM's sequence of the engine handle's comment above:
+     1. one silhouette launch on the static engine's stream, cars[0..n) in order (action 2 extracts into the slot's instance
+        frame; a fused car with action 0 or 1 gets an empty instance frame, white with depth 0, as ProcessSilhouette leaves it);
+     2. for every fused car: its stream waits for the static engine's, then b200_process_frame_async of its volume (pose and
+        intrinsics from cam, decay as below) with the slot's colour and depth renders;
+     3. b200_process_frame_async of the static map with static_view (normally d_depth and d_rgb after step 1), its depth render
+        into d_out_depth;
+     4. the static engine's stream waits for every slot that has work it has not waited for;
+     5. the static map's shaded raycast image and depth under the fused cars' layers, in cars order, dimmed and tinted as
+        b200_composite_instances does, into d_out_color / d_out_depth.
+   d_rgb / d_depth: the frame (img_w x img_h), updated in place by the silhouettes. decay: NULL, or {maxWeight, minAge} for
+   every volume. No host wait, no allocation, no copy from host memory. B200_ERR_INVALID, before anything is enqueued: a null
+   pointer, n < 0 or n > max_cars, a static view of another size, a slot out of range, a slot twice in one frame, a slot that
+   was never started, an unknown action or a mask it needs missing. Host counters are refreshed by b200_group_sync. */
+b200_status b200_group_frame_async(b200_group *g, b200_vec4u *d_rgb, float *d_depth, const b200_view *static_view,
+                                   const b200_group_car *cars, int n, const int32_t *decay, b200_vec4u *d_out_color,
+                                   float *d_out_depth);
+/* b200_sync of the static map and of every slot */
+b200_status b200_group_sync(b200_group *g);
 
 /* ---- evaluation consumer of the float raycast (SURVEY 8(f) rank 3): Evaluation::EvaluateDepth ----------------------------
    DS/Evaluation/Evaluation.cpp:241-304 with ProjectLidar (:214-238) and EvaluationCallback::ProcessLidarPoint /
