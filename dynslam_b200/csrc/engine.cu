@@ -212,16 +212,14 @@ static b200_status engine_create_body(const b200_engine_config *cfg, b200_engine
 // engine created after a variable was set or removed gets the new value (nothing is remembered per process).
 static void read_switches(b200_engine *e) {
   const char *v;
-  // default: V4 (packed-pair arithmetic, integrate.cu); B200_INTEGRATE_IMPL = v3 | tma | ldg select the earlier bit-exact variants,
-  // fast = V4 in tolerance mode (TSDF within 1 LSB of the 16-bit code, everything else bit-exact)
+  // default: V4 (packed-pair arithmetic, integrate.cu); B200_INTEGRATE_IMPL = v3 | tma select the other bit-exact kernels,
+  // fast = V4 in tolerance mode (TSDF within 1 LSB of the 16-bit code, everything else bit-exact); any other value is V4
   v = getenv("B200_INTEGRATE_IMPL");
-  e->integrateImpl = !v ? 3 : (v[0] == 'l' ? 0 : (v[0] == 't' ? 1 : (v[0] == 'f' ? 4 : ((v[0] == 'v' && v[1] == '3') ? 2 : 3))));
+  e->integrateImpl = !v ? 3 : (v[0] == 't' ? 1 : (v[0] == 'f' ? 4 : ((v[0] == 'v' && v[1] == '3') ? 2 : 3)));
   v = getenv("B200_V4_PPL"); e->pplV4 = (v && (atoi(v) == 1 || atoi(v) == 2)) ? atoi(v) : 0;
   v = getenv("B200_V4_TAIL"); e->v4TailFloor = (v && atoi(v) >= 1 && atoi(v) <= 6) ? atoi(v) : 3;
   v = getenv("B200_V3_PREFETCH"); e->v3Prefetch = v ? atoi(v) != 0 : true;
   v = getenv("B200_V3_CTAS"); e->ctasV3 = (v && (atoi(v) == 2 || atoi(v) == 4)) ? atoi(v) : 3;   // 3: 72 registers per thread; 4 = 56, 2 = 96
-  v = getenv("B200_INTEGRATE_REGS"); e->regsTma = (v && atoi(v) == 56) ? 56 : 48;
-  v = getenv("B200_INTEGRATE_CTAS"); e->ctasTma = v ? atoi(v) : 0;   // an upper bound; integrate_init_device sets the count
   v = getenv("B200_RC_TILE"); e->rcTileLog2 = v ? atoi(v) : 3; if (e->rcTileLog2 < 0 || e->rcTileLog2 > 5) e->rcTileLog2 = 3;
   v = getenv("B200_RC_ORDER"); e->rcOrder = v ? atoi(v) : 1;
   v = getenv("B200_RC_IMPL"); e->rcImpl = (v && v[0] == 'o') ? 0 : 1;

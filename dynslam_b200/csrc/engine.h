@@ -98,14 +98,13 @@ struct b200_engine {
   unsigned long long *d_dbg;          // timestamps written by instrumented kernels while the launch trace is on (b200_diag_read_debug)
   long long launches;
   int lastNoIntegrated;
-  int integrateImpl;                  // 0 = LDG variant, 1 = TMA bulk-copy variant (env B200_INTEGRATE_IMPL=ldg|tma)
+  int integrateImpl;                  // 1 = TMA kernel, 2 = V3, 3 = V4, 4 = V4 in tolerance mode (env B200_INTEGRATE_IMPL=tma|v3|v4|fast)
   // run-time switches, read from the environment when the engine is created (defaults when unset; README)
   int pplV4;                          // B200_V4_PPL=1|2 forces V4's two- / four-voxels-per-lane form; 0: by list length
   int v4TailFloor;                    // B200_V4_TAIL=1..6: blocks a V4 CTA keeps in flight when the list runs out (3)
   bool v3Prefetch;                    // B200_V3_PREFETCH=0 turns off the L2 prefetch of the images in V3 / V4
   int ctasV3;                         // B200_V3_CTAS=2|3|4: resident V3 CTAs per SM (3)
-  int regsTma;                        // B200_INTEGRATE_REGS=56: the 56-register TMA build (48)
-  int ctasTma;                        // TMA CTAs per SM: occupancy, at most 4, lowered by B200_INTEGRATE_CTAS
+  int ctasTma;                        // TMA CTAs per SM: occupancy of k_integrate_tma48, at most 4
   int rcTileLog2, rcOrder, rcImpl;    // B200_RC_TILE=0..5 (3: 8x4), B200_RC_ORDER=0|1 (1), B200_RC_IMPL=old (1: neighbourhood cache)
   int lastIntegrateKernel, lastIntegrateGrid;   // what the last launch_integrate ran (b200_diag_last_integrate)
   bool hostAuthoritative;            // host copies of the counters are newer than the device ones

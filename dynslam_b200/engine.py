@@ -227,7 +227,7 @@ class Engine:
         self.lib.b200_diag_set_grid_scale(self.h, int(k))
 
     def last_integrate(self):
-        """test hook (include/b200fusion_diag.h): (kernel, grid) of the last integrate launch; kernel 0 LDG, 1 TMA, 2 V3, 3 V4 with
+        """test hook (include/b200fusion_diag.h): (kernel, grid) of the last integrate launch; kernel 1 TMA, 2 V3, 3 V4 with
         two voxels per lane, 4 V4 with four, + 8 in tolerance mode"""
         k, g = C.c_int(), C.c_int()
         self.lib.b200_diag_last_integrate(self.h, C.byref(k), C.byref(g))

@@ -56,9 +56,10 @@ void b200_diag_set_max_rendering_blocks(b200_engine *e, int n);
    engine shares the device. k <= 1 restores the default. */
 void b200_diag_set_grid_scale(b200_engine *e, int k);
 
-/* The IntegrateIntoScene kernel that this engine's last integrate launch ran, and its grid (CTAs): 0 = LDG, 1 = TMA, 2 = V3,
+/* The IntegrateIntoScene kernel that this engine's last integrate launch ran, and its grid (CTAs): 1 = TMA, 2 = V3,
    3 = V4 with two voxels per lane, 4 = V4 with four voxels per lane; + 8 in tolerance mode (B200_INTEGRATE_IMPL=fast).
-   -1 and 0 before the first launch. Tests use it to check that the variant they mean to exercise really ran. */
+   Id 0 is no longer produced. -1 and 0 before the first launch. Tests use it to check that the variant they mean to
+   exercise really ran. */
 void b200_diag_last_integrate(const b200_engine *e, int *kernel, int *grid);
 
 /* Seed the decay queue the way AllocateSceneFromDepth does (Reco_CUDA.cu:302-316), without an allocation: the n block

@@ -79,12 +79,14 @@ def test_config1_plane_8mm():
 
 
 def test_integrate_ldg_variant_matches():
+    """`ldg` named a kernel of earlier versions: the value now selects V4, which matches the oracle"""
     os.environ["B200_INTEGRATE_IMPL"] = "ldg"
     try:
         pair, _ = P.run_sequence(P.Cfg(frames=5, raycast=False, decay=(1, 2)))
     finally:
         os.environ.pop("B200_INTEGRATE_IMPL", None)
     assert pair.rs.noVisibleBlocks > 1000
+    assert pair.eng.last_integrate()[0] == 3   # V4, two voxels per lane
 
 
 def test_integrate_v3_variant_matches():

@@ -7,7 +7,7 @@ Per trajectory: the stepwise path against the CPU oracle after every stage, with
 resets and deletes blocks re-observed from another side; the chained frame (decay swept in the raycast grid), its graph form
 and the pipelined host frames against the stepwise run; renders of all five types and the host-bound free-view preview from
 the last camera turned 90 and 180 degrees against the oracle. On `reverse` and `pitch_roll` also the old raycast, both
-raycast dispatch orders with the principal point above and right of the image, the v3 / tma / ldg integrate kernels and the
+raycast dispatch orders with the principal point above and right of the image, the v3 / tma integrate kernels and the
 tolerance-mode kernel under its one-LSB bar. The tolerance mode and the preview, which have no bit-exact twin, are checked
 against the analytic scene in float64."""
 import ctypes as C
@@ -177,7 +177,7 @@ def test_raycast_orders_off_image_principal_point(name, order):
         eng.close()
 
 
-@pytest.mark.parametrize("impl", ["v3", "tma", "ldg"])
+@pytest.mark.parametrize("impl", ["v3", "tma"])
 @pytest.mark.parametrize("name", SWITCHED)
 def test_integrate_kernels_equal_oracle(name, impl):
     switches, kernel = IMPLS[impl]

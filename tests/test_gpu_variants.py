@@ -21,12 +21,11 @@ from tests import parity as P
 pytestmark = pytest.mark.gpu
 
 # b200_diag_last_integrate's kernel ids
-LDG, TMA, V3, V4_PPL1, V4_PPL2, FAST = 0, 1, 2, 3, 4, 8
+TMA, V3, V4_PPL1, V4_PPL2, FAST = 1, 2, 3, 4, 8
 IMPLS = {"v4ppl1": (dict(B200_INTEGRATE_IMPL="v4", B200_V4_PPL=1), V4_PPL1),
          "v4ppl2": (dict(B200_INTEGRATE_IMPL="v4", B200_V4_PPL=2), V4_PPL2),
          "v3": (dict(B200_INTEGRATE_IMPL="v3"), V3),
-         "tma": (dict(B200_INTEGRATE_IMPL="tma"), TMA),
-         "ldg": (dict(B200_INTEGRATE_IMPL="ldg"), LDG)}
+         "tma": (dict(B200_INTEGRATE_IMPL="tma"), TMA)}
 
 
 @contextlib.contextmanager
@@ -201,7 +200,7 @@ def test_tolerance_mode_four_voxel_form():
 
 
 # ---- 3. approximate integration in the other kernels and in the fused frame --------------------------------------------
-@pytest.mark.parametrize("impl", ["v3", "tma", "ldg"])
+@pytest.mark.parametrize("impl", ["v3", "tma"])
 def test_approximate_integration_other_impls(impl):
     switches, kernel = IMPLS[impl]
     pair = run(P.Cfg(frames=4, frame_step=1, raycast=False, decay=(1, 2), requiresFullRendering=False), **switches)
